@@ -23,7 +23,6 @@ import json
 import os
 import warnings
 import zlib
-from collections import OrderedDict
 from types import SimpleNamespace
 from typing import List, Optional, Sequence
 
@@ -33,6 +32,7 @@ import torch
 from . import lib as L
 from . import parallel
 from . import synth
+from .blocks import GraphCache
 from .schedulers import DDIMScheduler, DDPMScheduler
 from .stft import TacotronSTFT
 from .t5 import T5EncoderModel
@@ -132,7 +132,7 @@ class AudioDiffusion:
         self.text_encoder = None
         self.allow_synthetic_tokenizer = allow_synthetic_tokenizer   # tests / synthetic weights only (see below)
         self._uncond_cache = {}
-        self._state = OrderedDict()   # captured CUDA graphs + their persistent I/O buffers, LRU-bounded
+        self._state = GraphCache(self.MAX_GRAPHS)   # captured UNet steps + their persistent I/O buffers
         self._temb_cache = {}
         self.last_step_ms: Optional[float] = None
         self.last_kernel_launches = 0
@@ -359,19 +359,11 @@ class AudioDiffusion:
         # and the generation of the packed weights the graph points into
         key = (Bu, H, W, prompt_embeds.shape[1], boolean_prompt_mask is not None, bool(cfg_on), str(device),
                unet.pack_generation) + tuple((f.shape[1], m is not None) for f, m in extra_streams)
-        st = self._state.get(key)
-        if st is not None:
-            self._state.move_to_end(key)
-        if st is None:
-            while len(self._state) >= self.MAX_GRAPHS:
-                self._state.popitem(last=False)
-            st = SimpleNamespace(
-                x_in=torch.zeros(Bu * HW, Cl * s, device=device, dtype=torch.bfloat16),
-                model_out=torch.zeros(Bu * HW, unet.config["out_channels"], device=device, dtype=torch.float32),
-                temb_cur=torch.zeros(Bu, temb_table.shape[1], device=device, dtype=torch.float32),
-                ident=torch.tensor([0, 0, 0, 1, 0, 0, 0, 0, 0, 1], device=device, dtype=torch.float32),
-                graph=None, per_forward=0)
-            self._state[key] = st
+        st = self._state.entry(key, lambda: dict(
+            x_in=torch.zeros(Bu * HW, Cl * s, device=device, dtype=torch.bfloat16),
+            model_out=torch.zeros(Bu * HW, unet.config["out_channels"], device=device, dtype=torch.float32),
+            temb_cur=torch.zeros(Bu, temb_table.shape[1], device=device, dtype=torch.float32),
+            ident=torch.tensor([0, 0, 0, 1, 0, 0, 0, 0, 0, 1], device=device, dtype=torch.float32)))
         x_in, model_out, temb_cur = st.x_in, st.model_out, st.temb_cur
         so = Cl if unet.split else 0
         # pack the initial latents into the (CFG-duplicated) channels-last bf16 UNet input
@@ -384,18 +376,11 @@ class AudioDiffusion:
         graph = None
         per_forward = 0
         if self.use_cuda_graph:
+            # the whole UNet forward (~400 launches) is captured once per shape; all its operands live in persistent
+            # buffers, so later calls only refresh their contents and replay
             if st.graph is None:
-                # the whole UNet forward (~400 launches) is captured once per shape; all its operands live in
-                # persistent buffers, so later calls only refresh their contents and replay
-                temb_cur.copy_(temb_table[0:1].expand_as(temb_cur))
-                n0 = L.launch_count()
-                run_unet()  # warm-up: allocates every scratch buffer, sets kernel attributes
-                st.per_forward = L.launch_count() - n0
-                torch.cuda.synchronize()
-                st.graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(st.graph):
-                    run_unet()
-            graph, per_forward = st.graph, st.per_forward
+                temb_cur.copy_(temb_table[0:1].expand_as(temb_cur))   # input of the warm-up run
+            graph, per_forward = self._state.capture(st, run_unet), st.launches
         self.launches_per_forward = per_forward
         n_eager0 = L.launch_count()
 

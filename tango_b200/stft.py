@@ -26,8 +26,8 @@ import numpy as np
 import torch
 
 from . import lib as L
+from .blocks import Buffers
 from .ops import PackedConv, ceil_div
-from .unet import _Buffers
 
 FLOOR = 1e-5   # dynamic_range_compression clip_val (audio_processing.py:85-91)
 
@@ -86,7 +86,7 @@ class TacotronSTFT:
         self.mel_basis_source = "slaney formula (not pinned against librosa)"
         self._device = torch.device("cpu")
         self._packed = False
-        self._bufs: Optional[_Buffers] = None
+        self._bufs: Optional[Buffers] = None
 
     # ------------------------------------------------------------------------------------------ module plumbing
     def to(self, device=None, *_a, **_k):
@@ -142,11 +142,8 @@ class TacotronSTFT:
         mel = torch.zeros(self.n_mel_channels, self.c_pad)
         mel[:, :self.bins] = self.mel_basis
         self._mel = PackedConv(mel, None, split=True, device=dev)
-        self._bufs = _Buffers(dev)
+        self._bufs = Buffers(dev)
         self._packed = True
-
-    def _buf(self, name, shape, dtype):
-        return self._bufs.get(name, shape, dtype)
 
     # ------------------------------------------------------------------------------------------ forward
     def mel_rows(self, y: torch.Tensor):
@@ -161,8 +158,8 @@ class TacotronSTFT:
             raise L.TangoB200Error(f"waveform of {T} samples is too short for reflect padding by {pad}")
         frames = 1 + T // hop                                    # conv1d output length over T + filter_length samples
         ld = ceil_div(T + 2 * pad, 8) * 8
-        hi = self._buf("hi", (B, ld), torch.bfloat16)
-        lo = self._buf("lo", (B, ld), torch.bfloat16)
+        hi = self._bufs.get("hi", (B, ld), torch.bfloat16)
+        lo = self._bufs.get("lo", (B, ld), torch.bfloat16)
         L.stft_frames(y, pad, hi, lo)
         rows = B * frames
         # STFT.transform (stft.py:52-83): every frame is a window of the padded signal, so the A operand of the basis
@@ -170,16 +167,16 @@ class TacotronSTFT:
         views = [L.View(t, FL, frames, 1, B, hop, ld, ld) for t in (hi, lo)]
         nkb, kh = FL // 64, self._basis.k_half
         groups = [(0, 0, 0, 0, 0, nkb), (1, 0, 0, 0, 0, nkb), (0, 0, 0, 0, kh, nkb)]   # hi*w_hi + lo*w_hi + hi*w_lo
-        Fq = self._buf("F", (rows, self.n_pad), torch.float32)
+        Fq = self._bufs.get("F", (rows, self.n_pad), torch.float32)
         L.conv_gemm(views, groups, self._basis.weight, frames, 1, B, out_f32=Fq, algo_k=FL)
-        mag = self._buf("mag", (rows, 2 * self.c_pad), torch.bfloat16)    # [hi | lo], pad columns stay zero
-        log_mag = self._buf("log_mag", (rows, self.bins), torch.float32)
-        energy = self._buf("energy", (rows,), torch.float32)
+        mag = self._bufs.get("mag", (rows, 2 * self.c_pad), torch.bfloat16)    # [hi | lo], pad columns stay zero
+        log_mag = self._bufs.get("log_mag", (rows, self.bins), torch.float32)
+        energy = self._bufs.get("energy", (rows,), torch.float32)
         L.stft_magnitude(Fq, self.bins, mag, self.c_pad, log_mag, energy, FLOOR)
         from .ops import run_linear
-        mel_lin = self._buf("mel_lin", (rows, self.n_mel_channels), torch.float32)
+        mel_lin = self._bufs.get("mel_lin", (rows, self.n_mel_channels), torch.float32)
         run_linear(self._mel, mag, out_f32=mel_lin)
-        mel = self._buf("mel", (rows, self.n_mel_channels), torch.float32)
+        mel = self._bufs.get("mel", (rows, self.n_mel_channels), torch.float32)
         L.log_clamp(mel_lin, mel, FLOOR)
         return mel, log_mag, energy, frames
 

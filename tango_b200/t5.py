@@ -23,6 +23,7 @@ from typing import Dict, Optional
 import torch
 
 from . import lib as L
+from .blocks import GraphCache
 from .ops import PackedConv, run_linear
 
 
@@ -76,7 +77,7 @@ class T5EncoderModel:
         self._sd: Optional[Dict[str, torch.Tensor]] = None
         self._packed = False
         self._relbias = {}
-        self._graphs = {}
+        self._graphs = GraphCache(8)
         self.use_cuda_graph = True      # one graph per (batch, padded length); off under the CPU orchestration tests
 
     # ----------------------------------------------------------------------------------------- transformers-style API
@@ -158,7 +159,7 @@ class T5EncoderModel:
             b.ff2 = PackedConv(sd[p + "1.DenseReluDense.wo.weight"], None, split=sp, device=dev)
             self.blocks.append(b)
         self._relbias = {}
-        self._graphs = {}
+        self._graphs.clear()
         self._packed = True
 
     def _relbias_for(self, L_: int) -> torch.Tensor:
@@ -184,22 +185,16 @@ class T5EncoderModel:
             raise IndexError(f"token id out of range [0, {cfg['vocab_size']}): min {lo}, max {hi}")
         d, H, ff = cfg["d_model"], cfg["num_heads"], cfg["d_ff"]
         inner, rows, eps = H * 64, B * Lt, float(cfg["layer_norm_epsilon"])
-        key = (B, Lt, attention_mask is not None)
-        st = self._graphs.get(key)
-        if st is None:
-            # persistent operands: the ~170 launches of the stack are captured once per (batch, length) into a CUDA graph
-            st = SimpleNamespace(
-                ids=torch.zeros(rows, device=dev, dtype=torch.int64),
-                kbias=torch.zeros(B, Lt, device=dev, dtype=torch.float32) if attention_mask is not None else None,
-                x=torch.empty(rows, d, device=dev, dtype=torch.float32),
-                n=torch.empty(rows, s * d, device=dev, dtype=torch.bfloat16),
-                qkv=torch.empty(rows, 3 * inner, device=dev, dtype=torch.float32),
-                ctx=torch.empty(rows, s * inner, device=dev, dtype=torch.bfloat16),
-                hff=torch.empty(rows, s * ff, device=dev, dtype=torch.bfloat16),
-                out=torch.empty(rows, d, device=dev, dtype=torch.float32), graph=None)
-            if len(self._graphs) >= 8:
-                self._graphs.pop(next(iter(self._graphs)))
-            self._graphs[key] = st
+        # persistent operands: the ~170 launches of the stack are captured once per (batch, length) into a CUDA graph
+        st = self._graphs.entry((B, Lt, attention_mask is not None), lambda: dict(
+            ids=torch.zeros(rows, device=dev, dtype=torch.int64),
+            kbias=torch.zeros(B, Lt, device=dev, dtype=torch.float32) if attention_mask is not None else None,
+            x=torch.empty(rows, d, device=dev, dtype=torch.float32),
+            n=torch.empty(rows, s * d, device=dev, dtype=torch.bfloat16),
+            qkv=torch.empty(rows, 3 * inner, device=dev, dtype=torch.float32),
+            ctx=torch.empty(rows, s * inner, device=dev, dtype=torch.bfloat16),
+            hff=torch.empty(rows, s * ff, device=dev, dtype=torch.bfloat16),
+            out=torch.empty(rows, d, device=dev, dtype=torch.float32)))
         st.ids.copy_(ids.view(-1))
         if st.kbias is not None:
             # get_extended_attention_mask: (1 - mask) * finfo.min, added to the position bias
@@ -225,13 +220,7 @@ class T5EncoderModel:
         if not (self.use_cuda_graph and dev.type == "cuda"):
             run()
         else:
-            if st.graph is None:
-                run()                                  # warm-up: kernel attributes
-                torch.cuda.synchronize()
-                st.graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(st.graph):
-                    run()
-            st.graph.replay()
+            self._graphs.capture(st, run).replay()
         return T5Output(st.out.view(B, Lt, d).clone())
 
     __call__ = forward

@@ -16,13 +16,14 @@ from __future__ import annotations
 
 import json
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional
 
 import torch
 
+from . import blocks
 from . import lib as L
-from . import ops
-from .ops import PackedConv, run_conv, run_linear
+from .blocks import Buffers, Packer, StatsArena
+from .ops import PackedConv, run_linear
 
 
 class UNetOutput(SimpleNamespace):
@@ -36,50 +37,6 @@ class _Cfg(dict):
 def _heads(cfg) -> List[int]:
     ahd = cfg["attention_head_dim"]
     return list(ahd) if isinstance(ahd, (list, tuple)) else [ahd] * len(cfg["block_out_channels"])
-
-
-class _Buffers:
-    """Named, shape-keyed scratch tensors (allocated once, reused by every forward — CUDA-graph friendly)."""
-
-    def __init__(self, device):
-        self.device = device
-        self.t: Dict[Tuple, torch.Tensor] = {}
-
-    def get(self, name: str, shape, dtype) -> torch.Tensor:
-        key = (name, tuple(shape), dtype)
-        buf = self.t.get(key)
-        if buf is None:
-            buf = torch.zeros(shape, device=self.device, dtype=dtype)
-            self.t[key] = buf
-        return buf
-
-
-class StatsArena:
-    """fp64 per-(image, channel) GroupNorm accumulators for every norm input of one forward, carved out of ONE buffer
-    so that a single fill zeroes them all at the start of the forward (slots keep their addresses: CUDA-graph safe).
-    A slot [NB, C, 2] belongs to one tensor; the GEMM that produces the tensor adds its column sums from the epilogue
-    (tng_conv_gemm gn_stats), the norm that consumes it — possibly twice: next layer and, as a skip connection, the up
-    path — reads them."""
-
-    def __init__(self, device, capacity: int):
-        self.buf = torch.zeros(max(capacity, 1), device=device, dtype=torch.float64)
-        self.slots: Dict[Tuple, Tuple[int, int]] = {}
-        self.used = 0
-
-    def slot(self, name: str, NB: int, C_: int) -> torch.Tensor:
-        key = (name, NB, C_)
-        hit = self.slots.get(key)
-        if hit is None:
-            n = NB * C_ * 2
-            if self.used + n > self.buf.numel():
-                raise L.TangoB200Error("GroupNorm statistics arena exhausted (internal sizing error)")
-            hit = (self.used, n)
-            self.slots[key] = hit
-            self.used += n
-        return self.buf[hit[0]:hit[0] + hit[1]].view(NB, C_, 2)
-
-    def zero(self):
-        self.buf[:max(self.used, 1)].zero_()
 
 
 class UNet2DConditionModel:
@@ -126,7 +83,7 @@ class UNet2DConditionModel:
         self._sd: Optional[Dict[str, torch.Tensor]] = None
         self._packed = False
         self.pack_generation = 0     # bumped whenever the packed weights / scratch buffers are rebuilt
-        self._bufs: Optional[_Buffers] = None
+        self._bufs: Optional[Buffers] = None
         self._cond = None
 
     # ----------------------------------------------------------------------------------------- diffusers-style API
@@ -179,23 +136,11 @@ class UNet2DConditionModel:
         cfg = self.config
         boc = cfg["block_out_channels"]
         P: Dict[str, object] = {}
-
-        def f32(k):
-            return sd[k].float().contiguous().to(dev)
-
-        def conv(p, **kw):
-            return PackedConv(sd[p + ".weight"], sd.get(p + ".bias"), split=sp, device=dev, **kw)
+        pk = Packer(sd, dev, sp)
+        f32, conv = pk.f32, pk.conv
 
         def resnet(p):
-            r = SimpleNamespace()
-            r.n1w, r.n1b, r.n2w, r.n2b = f32(p + ".norm1.weight"), f32(p + ".norm1.bias"), f32(p + ".norm2.weight"), f32(p + ".norm2.bias")
-            r.conv1 = conv(p + ".conv1")
-            if (p + ".conv_shortcut.weight") in sd:
-                r.conv2 = PackedConv(sd[p + ".conv2.weight"], sd[p + ".conv2.bias"], split=sp, device=dev,
-                                     sc_w=sd[p + ".conv_shortcut.weight"], sc_b=sd[p + ".conv_shortcut.bias"])
-            else:
-                r.conv2 = conv(p + ".conv2")
-            r.cin, r.cout = r.conv1.cin, r.conv1.cout
+            r = pk.resnet(p, "conv_shortcut", cfg.get("norm_eps", 1e-5))
             r.temb_w, r.temb_b = sd[p + ".time_emb_proj.weight"].float(), sd[p + ".time_emb_proj.bias"].float()
             return r
 
@@ -211,14 +156,13 @@ class UNet2DConditionModel:
             wqkv = torch.cat([sd[f"{b}.attn1.to_q.weight"], sd[f"{b}.attn1.to_k.weight"], sd[f"{b}.attn1.to_v.weight"]], 0)
             t.qkv = PackedConv(wqkv, None, split=sp, device=dev)
             t.out1 = conv(f"{b}.attn1.to_out.0")
-            t.q2 = PackedConv(sd[f"{b}.attn2.to_q.weight"], None, split=sp, device=dev)
+            t.q2 = conv(f"{b}.attn2.to_q")
             t.kv2 = PackedConv(torch.cat([sd[f"{b}.attn2.to_k.weight"], sd[f"{b}.attn2.to_v.weight"]], 0), None,
                                split=sp, device=dev)
             t.out2 = conv(f"{b}.attn2.to_out.0")
             cdim = t.proj_in.cout
             inner8 = 8 * cdim
-            t.ff1 = PackedConv(sd[f"{b}.ff.net.0.proj.weight"], sd[f"{b}.ff.net.0.proj.bias"], split=sp, device=dev,
-                               geglu_bn=256 if inner8 % 256 == 0 else 128)
+            t.ff1 = conv(f"{b}.ff.net.0.proj", geglu_bn=256 if inner8 % 256 == 0 else 128)
             t.ff2 = conv(f"{b}.ff.net.2")
             t.C = cdim
             return t
@@ -270,23 +214,17 @@ class UNet2DConditionModel:
         P["temb_b"] = torch.cat([r.temb_b for r in res_all], 0).contiguous().to(dev)
         P["transformers"] = [t for b in P["down"] for t in b.attns] + [P["mid"].attn] + [t for b in P["up"] for t in b.attns]
         P["n_extra"] = max((len(t.extra) for t in P["transformers"]), default=0)
-        # channels that carry GroupNorm statistics in one forward: conv_in, both convs of every resnet, every
-        # transformer output, the up / down sampler convs (sizes the statistics arenas, one per batch size)
         tr_all = list(P["transformers"]) + [x for t in P["transformers"] for x in t.extra]
-        P["stat_channels"] = (P["conv_in"].cout + sum(2 * r.cout for r in res_all) + sum(t.C for t in tr_all)
-                              + sum(b.down.cout for b in P["down"] if b.down is not None)
-                              + sum(b.up.cout for b in P["up"] if b.up is not None))
+        P["stat_channels"] = blocks.stat_channels(P["conv_in"], res_all, tr_all,
+                                                  [b.down for b in P["down"]] + [b.up for b in P["up"]])
         self.P = P
-        self._bufs = _Buffers(dev)
+        self._bufs = Buffers(dev)
         self._arenas: Dict[int, StatsArena] = {}
         self._cond = None
         self.pack_generation += 1
         self._packed = True
 
     # ----------------------------------------------------------------------------------------- building blocks
-    def _buf(self, name, shape, dtype):
-        return self._bufs.get(name, shape, dtype)
-
     def time_embedding_table(self, timesteps: torch.Tensor) -> torch.Tensor:
         """[n] timesteps -> [n, temb_total] fp32: every resnet's Linear(SiLU(TimestepEmbedding(t))) in one table
         (embeddings.py:22-62,200-212; resnet.py:572-573). Exact fp32 SIMT kernels; batch- and data-independent."""
@@ -317,17 +255,17 @@ class UNet2DConditionModel:
         Bu, Lk, D = ehs.shape
         s = self.s
         # persistent buffers (same addresses on every call with the same shapes -> a captured CUDA graph stays valid)
-        eb = self._buf("cond_ehs", (Bu * Lk, D * s), torch.bfloat16)
+        eb = self._bufs.get("cond_ehs", (Bu * Lk, D * s), torch.bfloat16)
         L.cast_act(ehs.view(Bu * Lk, D), 1, 1, Bu * Lk, eb, split_off=D if self.split else 0)
         kvs = []
         for i, t in enumerate(self.P["transformers"]):
-            kv = self._buf(f"cond_kv{i}", (Bu * Lk, 2 * t.C * s), torch.bfloat16)
+            kv = self._bufs.get(f"cond_kv{i}", (Bu * Lk, 2 * t.C * s), torch.bfloat16)
             run_linear(t.kv2, eb, out_bf16=kv)
             kvs.append(kv)
         bias = None
         if encoder_attention_mask is not None:
             m = encoder_attention_mask.to(self.device, non_blocking=True)
-            bias = self._buf("cond_bias", (Bu, Lk), torch.float32)
+            bias = self._bufs.get("cond_bias", (Bu, Lk), torch.float32)
             if m.dtype is torch.bool:
                 bias.copy_((1 - m.to(torch.float32)) * -10000.0)
             else:
@@ -338,17 +276,17 @@ class UNet2DConditionModel:
             if f.shape[0] != Bu or f.shape[2] != D:
                 raise L.TangoB200Error("extra conditioning streams must share the batch and feature width of the text states")
             Ln = f.shape[1]
-            fb = self._buf(f"cond_x{n}", (Bu * Ln, D * s), torch.bfloat16)
+            fb = self._bufs.get(f"cond_x{n}", (Bu * Ln, D * s), torch.bfloat16)
             L.cast_act(f.view(Bu * Ln, D), 1, 1, Bu * Ln, fb, split_off=D if self.split else 0)
             xk = []
             for i, t in enumerate(self.P["transformers"]):
-                kvn = self._buf(f"cond_x{n}kv{i}", (Bu * Ln, 2 * t.C * s), torch.bfloat16)
+                kvn = self._bufs.get(f"cond_x{n}kv{i}", (Bu * Ln, 2 * t.C * s), torch.bfloat16)
                 run_linear(t.extra[n].kv2, fb, out_bf16=kvn)
                 xk.append(kvn)
             xb = None
             if fmask is not None:
                 m = fmask.to(self.device, non_blocking=True)
-                xb = self._buf(f"cond_x{n}bias", (Bu, Ln), torch.float32)
+                xb = self._bufs.get(f"cond_x{n}bias", (Bu, Ln), torch.float32)
                 xb.copy_((1 - m.to(torch.float32)) * -10000.0 if m.dtype is torch.bool else m.to(torch.float32))
             extra.append(SimpleNamespace(kvs=xk, bias=xb, Lk=Ln))
         self._cond = SimpleNamespace(kvs=kvs, bias=bias, Bu=Bu, Lk=Lk, extra=extra)
@@ -357,31 +295,9 @@ class UNet2DConditionModel:
         a = self._arenas.get(NB)
         if a is None:
             # 1.5x: under the CFG shared prefix a few tensors exist at half batch AND full batch
-            a = StatsArena(self.device, int(1.5 * 2 * NB * self.P["stat_channels"]) + 4096)
+            a = StatsArena(self.device, NB, self.P["stat_channels"], headroom=1.5)
             self._arenas[NB] = a
         return a
-
-    def _resnet(self, name, r, x0, st0, x1, st1, NB, H, W, temb, temb_ld, ar: StatsArena):
-        """ResnetBlock2D (resnet.py:549-597) on rows; x0 / x1 (skip, may be None) arrive with their per-channel GroupNorm
-        statistics st0 / st1; returns (out, statistics of out)."""
-        R, HW, s, sp = NB * H * W, H * W, self.s, self.split
-        cin = r.cin
-        a1 = self._buf("a", (R, cin * s), torch.bfloat16)
-        has_sc = r.conv2.cin_sc > 0
-        raw = self._buf("raw", (R, cin * s), torch.bfloat16) if has_sc else None
-        eps = self.config.get("norm_eps", 1e-5)
-        L.groupnorm(x0, st0, x1, st1, NB, HW, 32, r.n1w, r.n1b, eps, L.ACT_SILU, a1, split_off=cin if sp else 0, raw=raw,
-                    raw_split_off=cin if sp else 0)
-        h1 = self._buf("h1", (R, r.cout), torch.float32)
-        st_h1 = ar.slot(name + "_h1", NB, r.cout)
-        run_conv(r.conv1, a1, NB, H, W, rowvec=temb[:, r.temb_off:], rowvec_ld=temb_ld, out_f32=h1, gn_stats=st_h1,
-                 stats_hw=HW)
-        a2 = self._buf("a", (R, r.cout * s), torch.bfloat16)
-        L.groupnorm(h1, st_h1, None, None, NB, HW, 32, r.n2w, r.n2b, eps, L.ACT_SILU, a2, split_off=r.cout if sp else 0)
-        out = self._buf(name, (R, r.cout), torch.float32)
-        st_out = ar.slot(name, NB, r.cout)
-        run_conv(r.conv2, a2, NB, H, W, sc_x=raw, res=None if has_sc else x0, out_f32=out, gn_stats=st_out, stats_hw=HW)
-        return out, st_out
 
     def _transformer(self, name, t, x, st_x, NB, H, W, kv, bias, Lk, ar: StatsArena, shared_half: bool = False):
         """Transformer2DModel (transformer_2d.py:214-321) on rows; returns (out, statistics of out).
@@ -393,37 +309,37 @@ class UNet2DConditionModel:
         NBp = NB // 2 if shared_half else NB   # batch of the (possibly shared) prefix
         Rp, R = NBp * HW, NB * HW
         scale = 64 ** -0.5
-        a = self._buf("a", (Rp, Cc * s), torch.bfloat16)
+        a = self._bufs.get("a", (Rp, Cc * s), torch.bfloat16)
         L.groupnorm(x, st_x, None, None, NBp, HW, 32, t.nw, t.nb, 1e-6, L.ACT_NONE, a, split_off=so)
-        hs = self._buf("hs", (R, Cc), torch.float32)
+        hs = self._bufs.get("hs", (R, Cc), torch.float32)
         hsp = hs[:Rp]
         run_linear(t.proj_in, a, out_f32=hsp)
-        n = self._buf("ln", (R, Cc * s), torch.bfloat16)
+        n = self._bufs.get("ln", (R, Cc * s), torch.bfloat16)
         L.layernorm(hsp, t.ln1w, t.ln1b, 1e-5, n[:Rp], split_off=so)
-        qkv = self._buf("qkv", (R, 3 * Cc * s), torch.bfloat16)
+        qkv = self._bufs.get("qkv", (R, 3 * Cc * s), torch.bfloat16)
         run_linear(t.qkv, n[:Rp], out_bf16=qkv[:Rp])
-        ao = self._buf("ao", (R, Cc * s), torch.bfloat16)
+        ao = self._bufs.get("ao", (R, Cc * s), torch.bfloat16)
         L.attention(qkv[:Rp], qkv[:Rp], qkv[:Rp], ao[:Rp], batch=NBp, heads=t.heads, Lq=HW, Lk=HW, scale=scale, q_col0=0,
                     k_col0=Cc, v_col0=2 * Cc, nsplit=s, q_lo_off=3 * Cc, k_lo_off=3 * Cc, v_lo_off=3 * Cc, split_off=so)
         run_linear(t.out1, ao[:Rp], res=hsp, out_f32=hsp)
         if shared_half:
             hs[Rp:].copy_(hsp)          # second CFG half = first half up to here
-            xf = self._buf(name + "_xdup", (R, Cc), torch.float32)
+            xf = self._bufs.get(name + "_xdup", (R, Cc), torch.float32)
             xf[:Rp].copy_(x)
             xf[Rp:].copy_(x)
             x = xf
         L.layernorm(hs, t.ln2w, t.ln2b, 1e-5, n, split_off=so)
-        q = self._buf("q2", (R, Cc * s), torch.bfloat16)
+        q = self._bufs.get("q2", (R, Cc * s), torch.bfloat16)
         run_linear(t.q2, n, out_bf16=q)
         L.attention(q, kv, kv, ao, batch=NB, heads=t.heads, Lq=HW, Lk=Lk, scale=scale, q_col0=0, k_col0=0, v_col0=Cc,
                     kbias=bias, nsplit=s, q_lo_off=Cc, k_lo_off=2 * Cc, v_lo_off=2 * Cc, split_off=so)
         run_linear(t.out2, ao, res=hs, out_f32=hs)
         L.layernorm(hs, t.ln3w, t.ln3b, 1e-5, n, split_off=so)
-        ff = self._buf("ff", (R, 4 * Cc * s), torch.bfloat16)
+        ff = self._bufs.get("ff", (R, 4 * Cc * s), torch.bfloat16)
         run_linear(t.ff1, n, out_bf16=ff)
-        hsb = self._buf("hsb", (R, Cc * s), torch.bfloat16)
+        hsb = self._bufs.get("hsb", (R, Cc * s), torch.bfloat16)
         run_linear(t.ff2, ff, res=hs, out_bf16=hsb)
-        out = self._buf(name, (R, Cc), torch.float32)
+        out = self._bufs.get(name, (R, Cc), torch.float32)
         st_out = ar.slot(name, NB, Cc)
         run_linear(t.proj_out, hsb, res=x, out_f32=out, gn_stats=st_out, stats_hw=HW)
         return out, st_out
@@ -437,7 +353,7 @@ class UNet2DConditionModel:
         models.py:235): conv_in, the first resnet and the first transformer up to its self-attention output — everything
         before the first cross-attention — are then computed for one half only and duplicated."""
         self._pack()
-        P, cfg, s, sp = self.P, self.config, self.s, self.split
+        P, cfg, sp = self.P, self.config, self.split
         c = self._cond
         if c is None or c.Bu != NB:
             raise L.TangoB200Error("set_conditioning() must be called with the same batch before forward_rows()")
@@ -449,9 +365,12 @@ class UNet2DConditionModel:
         NBp = NB // 2 if shared else NB
         ar = self._arena(NB)
         ar.zero()                       # one fill for the GroupNorm statistics of the whole forward
-        h = self._buf("conv_in", (R, P["conv_in"].cout), torch.float32)
-        st = ar.slot("conv_in", NB, P["conv_in"].cout)
-        run_conv(P["conv_in"], x_in, NBp, H, W, out_f32=h[:NBp * H * W], gn_stats=st[:NBp], stats_hw=H * W)
+        bufs = self._bufs
+
+        def resnet(name, r, x, st_x, nb, skip=None, st_skip=None):
+            return blocks.resnet(bufs, ar, sp, name, r, x, st_x, nb, ch, cw, skip, st_skip, temb[:, r.temb_off:], temb_ld)
+
+        h, st = blocks.conv_in(bufs, ar, "conv_in", P["conv_in"], x_in, NB, H, W, NBp)
         if shared:
             h[NBp * H * W:].copy_(h[:NBp * H * W])   # the conv_in output is also a skip connection (full batch)
             st[NBp:].copy_(st[:NBp])
@@ -470,60 +389,43 @@ class UNet2DConditionModel:
             for j, r in enumerate(blk.resnets):
                 first = shared and i == 0 and j == 0
                 if first:
-                    hp, stp = self._resnet("d0r0", r, h[:NBp * H * W], st[:NBp], None, None, NBp, ch, cw, temb, temb_ld, ar)
+                    hp, stp = resnet("d0r0", r, h[:NBp * H * W], st[:NBp], NBp)
                     h, st = self._transformer("d0t0", blk.attns[0], hp, stp, NB, ch, cw, c.kvs[ti], c.bias, c.Lk, ar,
                                               shared_half=True)
                     h, st = extras("d0t0", blk.attns[0], h, st, ti)
                     ti += 1
                     skips.append((h, st))
                     continue
-                h, st = self._resnet(f"d{i}r{j}", r, h, st, None, None, NB, ch, cw, temb, temb_ld, ar)
+                h, st = resnet(f"d{i}r{j}", r, h, st, NB)
                 if blk.attns:
                     h, st = self._transformer(f"d{i}t{j}", blk.attns[j], h, st, NB, ch, cw, c.kvs[ti], c.bias, c.Lk, ar)
                     h, st = extras(f"d{i}t{j}", blk.attns[j], h, st, ti)
                     ti += 1
                 skips.append((h, st))
             if blk.down is not None:
-                Cc = blk.down.cin
-                xb = self._buf("a", (NB * ch * cw, Cc * s), torch.bfloat16)
-                L.cast_act(h, NB, ch, cw, xb, split_off=Cc if sp else 0)
-                hd = self._buf(f"d{i}ds", (NB * (ch // 2) * (cw // 2), blk.down.cout), torch.float32)
-                st = ar.slot(f"d{i}ds", NB, blk.down.cout)
-                run_conv(blk.down, xb, NB, ch, cw, out_f32=hd, gn_stats=st, stats_hw=(ch // 2) * (cw // 2))
+                h, st = blocks.downsample(bufs, ar, sp, f"d{i}ds", blk.down, h, NB, ch, cw)
                 ch, cw = ch // 2, cw // 2
-                h = hd
                 skips.append((h, st))
         m = P["mid"]
-        h, st = self._resnet("m0", m.r0, h, st, None, None, NB, ch, cw, temb, temb_ld, ar)
+        h, st = resnet("m0", m.r0, h, st, NB)
         h, st = self._transformer("mt", m.attn, h, st, NB, ch, cw, c.kvs[ti], c.bias, c.Lk, ar)
         h, st = extras("mt", m.attn, h, st, ti)
         ti += 1
-        h, st = self._resnet("m1", m.r1, h, st, None, None, NB, ch, cw, temb, temb_ld, ar)
+        h, st = resnet("m1", m.r1, h, st, NB)
         for i, blk in enumerate(P["up"]):
             for j, r in enumerate(blk.resnets):
                 skip, st_skip = skips.pop()
-                h, st = self._resnet(f"u{i}r{j}", r, h, st, skip, st_skip, NB, ch, cw, temb, temb_ld, ar)
+                h, st = resnet(f"u{i}r{j}", r, h, st, NB, skip, st_skip)
                 if blk.attns:
                     h, st = self._transformer(f"u{i}t{j}", blk.attns[j], h, st, NB, ch, cw, c.kvs[ti], c.bias, c.Lk, ar)
                     h, st = extras(f"u{i}t{j}", blk.attns[j], h, st, ti)
                     ti += 1
             if blk.up is not None:
-                Cc = blk.up.cin
-                xb = self._buf("a", (NB * 4 * ch * cw, Cc * s), torch.bfloat16)
-                L.cast_act(h, NB, ch, cw, xb, upsample2x=True, split_off=Cc if sp else 0)
+                h, st = blocks.upsample(bufs, ar, sp, f"u{i}us", blk.up, h, NB, ch, cw)
                 ch, cw = 2 * ch, 2 * cw
-                hu = self._buf(f"u{i}us", (NB * ch * cw, blk.up.cout), torch.float32)
-                st = ar.slot(f"u{i}us", NB, blk.up.cout)
-                run_conv(blk.up, xb, NB, ch, cw, out_f32=hu, gn_stats=st, stats_hw=ch * cw)
-                h = hu
-        Cc = cfg["block_out_channels"][0]
-        a = self._buf("a", (R, Cc * s), torch.bfloat16)
-        L.groupnorm(h, st, None, None, NB, H * W, 32, P["norm_out"][0], P["norm_out"][1], cfg.get("norm_eps", 1e-5),
-                    L.ACT_SILU, a, split_off=Cc if sp else 0)
         if out is None:
-            out = self._buf("unet_out", (R, P["conv_out"].cout), torch.float32)
-        run_conv(P["conv_out"], a, NB, H, W, out_f32=out)
-        return out
+            out = bufs.get("unet_out", (R, P["conv_out"].cout), torch.float32)
+        return blocks.norm_out(bufs, sp, h, st, NB, H, W, *P["norm_out"], cfg.get("norm_eps", 1e-5), P["conv_out"], out)
 
     # ----------------------------------------------------------------------------------------- reference-style call
     def input_rows(self, sample: torch.Tensor) -> torch.Tensor:

@@ -20,10 +20,11 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
+from . import blocks
 from . import lib as L
+from .blocks import Buffers, GraphCache, Packer, StatsArena
 from .ops import PackedConv, run_conv, run_linear
 from .synth import HIFIGAN_CONFIG, VAE_CONFIG, vae_decoder_param_shapes, vae_encoder_param_shapes
-from .unet import StatsArena, _Buffers
 
 
 class DiagonalGaussianDistribution:
@@ -110,24 +111,11 @@ class AutoencoderKL:
         L.load()
         sd, dev, sp = self._sd, self._device, self.split
         dd = self.ddconfig
-
-        def f32(k):
-            return sd[k].float().contiguous().to(dev)
-
-        def conv(p, **kw):
-            return PackedConv(sd[p + ".weight"], sd.get(p + ".bias"), split=sp, device=dev, **kw)
+        pk = Packer(sd, dev, sp)
+        f32, conv = pk.f32, pk.conv
 
         def res(p):
-            r = SimpleNamespace()
-            r.n1w, r.n1b, r.n2w, r.n2b = f32(p + ".norm1.weight"), f32(p + ".norm1.bias"), f32(p + ".norm2.weight"), f32(p + ".norm2.bias")
-            r.conv1 = conv(p + ".conv1")
-            if (p + ".nin_shortcut.weight") in sd:
-                r.conv2 = PackedConv(sd[p + ".conv2.weight"], sd[p + ".conv2.bias"], split=sp, device=dev,
-                                     sc_w=sd[p + ".nin_shortcut.weight"], sc_b=sd[p + ".nin_shortcut.bias"])
-            else:
-                r.conv2 = conv(p + ".conv2")
-            r.cin, r.cout = r.conv1.cin, r.conv1.cout
-            return r
+            return pk.resnet(p, "nin_shortcut", 1e-6)
 
         P = SimpleNamespace()
         # post_quant_conv with the 1/scale_factor of decode_first_stage folded in (autoencoder.py:116-124,60-61)
@@ -136,14 +124,7 @@ class AutoencoderKL:
         P.pq_b = f32("post_quant_conv.bias")
         P.conv_in = conv("decoder.conv_in")
         P.mid1, P.mid2 = res("decoder.mid.block_1"), res("decoder.mid.block_2")
-        a = "decoder.mid.attn_1"
-        P.attn = SimpleNamespace(nw=f32(a + ".norm.weight"), nb=f32(a + ".norm.bias"))
-        Cc = sd[a + ".q.weight"].shape[0]
-        wq = torch.cat([sd[a + ".q.weight"], sd[a + ".k.weight"], sd[a + ".v.weight"]], 0).reshape(3 * Cc, Cc)
-        bq = torch.cat([sd[a + ".q.bias"], sd[a + ".k.bias"], sd[a + ".v.bias"]], 0)
-        P.attn.qkv = PackedConv(wq, bq, split=sp, device=dev)
-        P.attn.proj = PackedConv(sd[a + ".proj_out.weight"].reshape(Cc, Cc), sd[a + ".proj_out.bias"], split=sp, device=dev)
-        P.attn.C = Cc
+        P.attn = pk.attn_block("decoder.mid.attn_1")
         P.up = []
         nres = len(dd["ch_mult"])
         for lvl in reversed(range(nres)):
@@ -157,7 +138,7 @@ class AutoencoderKL:
         # ---- vocoder
         h = self.hifigan
         V = SimpleNamespace()
-        V.conv_pre = PackedConv(sd["vocoder.conv_pre.weight"], sd["vocoder.conv_pre.bias"], split=sp, device=dev)
+        V.conv_pre = conv("vocoder.conv_pre")
         V.stages = []
         nk = len(h["resblock_kernel_sizes"])
         for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
@@ -171,54 +152,30 @@ class AutoencoderKL:
                 rb = SimpleNamespace(c1=[], c2=[])
                 p = f"vocoder.resblocks.{i * nk + j}"
                 for di, d in enumerate(h["resblock_dilation_sizes"][j]):
-                    rb.c1.append(PackedConv(sd[f"{p}.convs1.{di}.weight"], sd[f"{p}.convs1.{di}.bias"], split=sp,
-                                            device=dev, dilation=d))
-                    rb.c2.append(PackedConv(sd[f"{p}.convs2.{di}.weight"], sd[f"{p}.convs2.{di}.bias"], split=sp,
-                                            device=dev, dilation=1))
+                    rb.c1.append(conv(f"{p}.convs1.{di}", dilation=d))
+                    rb.c2.append(conv(f"{p}.convs2.{di}"))
                 st.blocks.append(rb)
             V.stages.append(st)
-        V.conv_post = PackedConv(sd["vocoder.conv_post.weight"], sd["vocoder.conv_post.bias"], split=sp, device=dev)
+        V.conv_post = conv("vocoder.conv_post")
         res_all = [P.mid1, P.mid2] + [r for blk in P.up for r in blk.res]
-        P.stat_channels = (P.conv_in.cout + sum(2 * r.cout for r in res_all) + P.attn.C
-                           + sum(blk.up.cout for blk in P.up if blk.up is not None))
+        P.stat_channels = blocks.stat_channels(P.conv_in, res_all, [P.attn], [blk.up for blk in P.up])
         self.P, self.V = P, V
-        self._bufs = _Buffers(dev)
+        self._bufs = Buffers(dev)
         self._arenas = {}
-        self._graphs = {}
+        self._graphs = GraphCache(4)
         self._packed = True
 
-    def _buf(self, name, shape, dtype):
-        return self._bufs.get(name, shape, dtype)
-
     def _arena(self, tag: str, NB: int, channels: int) -> StatsArena:
-        """GroupNorm statistics arena of one decode / encode call (see unet.StatsArena)."""
+        """GroupNorm statistics arena of one decode / encode call (see blocks.StatsArena)."""
         key = (tag, NB)
         a = self._arenas.get(key)
         if a is None:
-            a = StatsArena(self._device, 2 * NB * channels + 4096)
+            a = StatsArena(self._device, NB, channels)
             self._arenas[key] = a
         a.zero()
         return a
 
     # ------------------------------------------------------------------------------------------ decoder
-    def _resnet(self, name, r, x, st, NB, H, W, ar):
-        """modules.py:155-175 on rows; (x, st) = input and its per-channel GroupNorm statistics; returns (out, stats)."""
-        R, s, sp, HW = NB * H * W, self.s, self.split, H * W
-        a1 = self._buf("a", (R, r.cin * s), torch.bfloat16)
-        has_sc = r.conv2.cin_sc > 0
-        raw = self._buf("raw", (R, r.cin * s), torch.bfloat16) if has_sc else None
-        L.groupnorm(x, st, None, None, NB, HW, 32, r.n1w, r.n1b, 1e-6, L.ACT_SILU, a1, split_off=r.cin if sp else 0,
-                    raw=raw, raw_split_off=r.cin if sp else 0)
-        h1 = self._buf("h1", (R, r.cout), torch.float32)
-        st_h1 = ar.slot(name + "_h1", NB, r.cout)
-        run_conv(r.conv1, a1, NB, H, W, out_f32=h1, gn_stats=st_h1, stats_hw=HW)
-        a2 = self._buf("a", (R, r.cout * s), torch.bfloat16)
-        L.groupnorm(h1, st_h1, None, None, NB, HW, 32, r.n2w, r.n2b, 1e-6, L.ACT_SILU, a2, split_off=r.cout if sp else 0)
-        out = self._buf(name, (R, r.cout), torch.float32)
-        st_out = ar.slot(name, NB, r.cout)
-        run_conv(r.conv2, a2, NB, H, W, sc_x=raw, res=None if has_sc else x, out_f32=out, gn_stats=st_out, stats_hw=HW)
-        return out, st_out
-
     def _attn(self, x, st, NB, H, W, ar, t=None):
         """modules.py:204-230: softmax(q k^T / sqrt(C)) v over the H*W positions of each image, one head.
         `t`: packed attention weights (default: the decoder's mid block). Returns (out, stats of out)."""
@@ -226,23 +183,23 @@ class AutoencoderKL:
         R, HW, s, sp, Cc = NB * H * W, H * W, self.s, self.split, t.C
         if HW % 64:
             raise L.TangoB200Error("VAE attention needs H*W to be a multiple of 64")
-        a = self._buf("a", (R, Cc * s), torch.bfloat16)
+        a = self._bufs.get("a", (R, Cc * s), torch.bfloat16)
         L.groupnorm(x, st, None, None, NB, HW, 32, t.nw, t.nb, 1e-6, L.ACT_NONE, a, split_off=Cc if sp else 0)
-        qkv = self._buf("vqkv", (R, 3 * Cc * s), torch.bfloat16)  # [q k v | q_lo k_lo v_lo]
+        qkv = self._bufs.get("vqkv", (R, 3 * Cc * s), torch.bfloat16)  # [q k v | q_lo k_lo v_lo]
         run_linear(t.qkv, a, out_bf16=qkv)
-        o = self._buf("vo", (R, Cc * s), torch.bfloat16)
+        o = self._bufs.get("vo", (R, Cc * s), torch.bfloat16)
         if not sp and Cc == 512 and HW % 128 == 0:
             # perf mode: one flash-attention launch for the whole batch, the [HW, HW] scores never leave the SM
             L.attention_wide(qkv, qkv, qkv, o, batch=NB, L=HW, dim=Cc, scale=float(Cc) ** -0.5, q_col0=0, k_col0=Cc,
                              v_col0=2 * Cc)
-            out = self._buf("vattn", (R, Cc), torch.float32)
+            out = self._bufs.get("vattn", (R, Cc), torch.float32)
             st_out = ar.slot("vattn", NB, Cc)
             run_linear(t.proj, o, res=x, out_f32=out, gn_stats=st_out, stats_hw=HW)
             return out, st_out
         # parity mode (hi/lo split operands): scores through HBM, image by image — GEMM -> row softmax -> GEMM
-        S = self._buf("vS", (HW, HW), torch.float32)
-        Pm = self._buf("vP", (HW, HW * s), torch.bfloat16)
-        vt = self._buf("vVt", (Cc, HW * s), torch.bfloat16)
+        S = self._bufs.get("vS", (HW, HW), torch.float32)
+        Pm = self._bufs.get("vP", (HW, HW * s), torch.bfloat16)
+        vt = self._bufs.get("vVt", (Cc, HW * s), torch.bfloat16)
         nkb_c, nkb_hw = Cc // 64, HW // 64
         lo = 3 * Cc
         for b in range(NB):
@@ -266,7 +223,7 @@ class AutoencoderKL:
                 g = [(0, 0, 0, 0, 0, nkb_hw)]
             ob = o[b * HW:(b + 1) * HW]
             L.conv_gemm([pv], g, vt, HW, 1, 1, out_bf16=ob, split_off=Cc if sp else 0)
-        out = self._buf("vattn", (R, Cc), torch.float32)
+        out = self._bufs.get("vattn", (R, Cc), torch.float32)
         st_out = ar.slot("vattn", NB, Cc)
         run_linear(t.proj, o, res=x, out_f32=out, gn_stats=st_out, stats_hw=HW)
         return out, st_out
@@ -277,67 +234,43 @@ class AutoencoderKL:
         P, s, sp = self.P, self.s, self.split
         R = NB * H * W
         zc = P.pq_w.shape[0]
-        z1 = self._buf("vz", (R, zc), torch.float32)
+        z1 = self._bufs.get("vz", (R, zc), torch.float32)
         L.linear_f32(z_rows, P.pq_w, P.pq_b, z1)
-        zb = self._buf("vzb", (R, zc * s), torch.bfloat16)
+        zb = self._bufs.get("vzb", (R, zc * s), torch.bfloat16)
         L.cast_act(z1, NB, H, W, zb, split_off=zc if sp else 0)
         ar = self._arena("dec", NB, P.stat_channels)
-        h = self._buf("vconv_in", (R, P.conv_in.cout), torch.float32)
-        st = ar.slot("vconv_in", NB, P.conv_in.cout)
-        run_conv(P.conv_in, zb, NB, H, W, out_f32=h, gn_stats=st, stats_hw=H * W)
-        h, st = self._resnet("vmid1", P.mid1, h, st, NB, H, W, ar)
+        bufs = self._bufs
+        h, st = blocks.conv_in(bufs, ar, "vconv_in", P.conv_in, zb, NB, H, W)
+        h, st = blocks.resnet(bufs, ar, sp, "vmid1", P.mid1, h, st, NB, H, W)
         h, st = self._attn(h, st, NB, H, W, ar)
-        h, st = self._resnet("vmid2", P.mid2, h, st, NB, H, W, ar)
+        h, st = blocks.resnet(bufs, ar, sp, "vmid2", P.mid2, h, st, NB, H, W)
         ch, cw = H, W
         for li, blk in enumerate(P.up):
             for bi, r in enumerate(blk.res):
-                h, st = self._resnet(f"vup{li}_{bi}", r, h, st, NB, ch, cw, ar)
+                h, st = blocks.resnet(bufs, ar, sp, f"vup{li}_{bi}", r, h, st, NB, ch, cw)
             if blk.up is not None:
-                Cc = blk.up.cin
-                xb = self._buf("a", (NB * 4 * ch * cw, Cc * s), torch.bfloat16)
-                L.cast_act(h, NB, ch, cw, xb, upsample2x=True, split_off=Cc if sp else 0)
+                h, st = blocks.upsample(bufs, ar, sp, f"vups{li}", blk.up, h, NB, ch, cw)
                 ch, cw = 2 * ch, 2 * cw
-                hu = self._buf(f"vups{li}", (NB * ch * cw, blk.up.cout), torch.float32)
-                st = ar.slot(f"vups{li}", NB, blk.up.cout)
-                run_conv(blk.up, xb, NB, ch, cw, out_f32=hu, gn_stats=st, stats_hw=ch * cw)
-                h = hu
-        Cc = h.shape[1]
-        a = self._buf("a", (NB * ch * cw, Cc * s), torch.bfloat16)
-        L.groupnorm(h, st, None, None, NB, ch * cw, 32, P.no_w, P.no_b, 1e-6, L.ACT_SILU, a, split_off=Cc if sp else 0)
-        mel = self._buf("vmel", (NB * ch * cw, P.conv_out.cout), torch.float32)
-        run_conv(P.conv_out, a, NB, ch, cw, out_f32=mel)
-        return mel
+        mel = bufs.get("vmel", (NB * ch * cw, P.conv_out.cout), torch.float32)
+        return blocks.norm_out(bufs, sp, h, st, NB, ch, cw, P.no_w, P.no_b, 1e-6, P.conv_out, mel)
 
     def decode_rows_to_waveform(self, z_rows: torch.Tensor, NB: int, H: int, W: int, use_cuda_graph: bool = True):
         """decode_first_stage + decode_to_waveform on rows: fp32 [NB*H*W, 8] latents -> (wave fp32 [NB, L], int16
         [NB, L]) on the device. The ~600 launches of the decoder and the vocoder are captured once per shape into a CUDA
         graph (all operands live in persistent buffers) and replayed afterwards."""
         self._pack()
-        if not use_cuda_graph:
-            mel = self.decode_rows(z_rows, NB, H, W)
+
+        def run(z):
+            mel = self.decode_rows(z, NB, H, W)
             return self.vocoder_rows(mel.view(NB * 4 * H, 4 * W), NB, 4 * H)
-        key = (NB, H, W)
-        st = self._graphs.get(key)
-        if st is None:
-            zin = self._buf("graph_zin", tuple(z_rows.shape), torch.float32)
-            zin.copy_(z_rows)
 
-            def run():
-                mel = self.decode_rows(zin, NB, H, W)
-                return self.vocoder_rows(mel.view(NB * 4 * H, 4 * W), NB, 4 * H)
-
-            run()                               # warm-up: allocates every scratch buffer, sets kernel attributes
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                wf, wi = run()
-            st = SimpleNamespace(graph=g, zin=zin, wf=wf, wi=wi)
-            if len(self._graphs) >= 4:
-                self._graphs.pop(next(iter(self._graphs)))
-            self._graphs[key] = st
+        if not use_cuda_graph:
+            return run(z_rows)
+        st = self._graphs.entry((NB, H, W),
+                                lambda: dict(zin=self._bufs.get("graph_zin", tuple(z_rows.shape), torch.float32)))
         st.zin.copy_(z_rows)
-        st.graph.replay()
-        return st.wf, st.wi
+        self._graphs.capture(st, lambda: run(st.zin)).replay()
+        return st.outputs
 
     def decode_first_stage(self, z: torch.Tensor, predict_cids=False, force_not_quantize=False) -> torch.Tensor:
         """(B, 8, T/4, 16) latents -> (B, 1, T, 64) log-mel (autoencoder.py:116-124)."""
@@ -362,24 +295,11 @@ class AutoencoderKL:
         if self._esd is None:
             raise L.TangoB200Error("AutoencoderKL was loaded without encoder.* / quant_conv.* weights")
         sd, dev, sp, dd = self._esd, self._device, self.split, self.ddconfig
-
-        def f32(k):
-            return sd[k].float().contiguous().to(dev)
-
-        def conv(p, **kw):
-            return PackedConv(sd[p + ".weight"], sd.get(p + ".bias"), split=sp, device=dev, **kw)
+        pk = Packer(sd, dev, sp)
+        f32, conv = pk.f32, pk.conv
 
         def res(p):
-            r = SimpleNamespace()
-            r.n1w, r.n1b, r.n2w, r.n2b = f32(p + ".norm1.weight"), f32(p + ".norm1.bias"), f32(p + ".norm2.weight"), f32(p + ".norm2.bias")
-            r.conv1 = conv(p + ".conv1")
-            if (p + ".nin_shortcut.weight") in sd:
-                r.conv2 = PackedConv(sd[p + ".conv2.weight"], sd[p + ".conv2.bias"], split=sp, device=dev,
-                                     sc_w=sd[p + ".nin_shortcut.weight"], sc_b=sd[p + ".nin_shortcut.bias"])
-            else:
-                r.conv2 = conv(p + ".conv2")
-            r.cin, r.cout = r.conv1.cin, r.conv1.cout
-            return r
+            return pk.resnet(p, "nin_shortcut", 1e-6)
 
         E = SimpleNamespace()
         w_in = sd["encoder.conv_in.weight"].float()
@@ -394,21 +314,13 @@ class AutoencoderKL:
                 blk.down = conv(f"encoder.down.{lvl}.downsample.conv", stride=2, pad=0)
             E.down.append(blk)
         E.mid1, E.mid2 = res("encoder.mid.block_1"), res("encoder.mid.block_2")
-        a = "encoder.mid.attn_1"
-        E.attn = SimpleNamespace(nw=f32(a + ".norm.weight"), nb=f32(a + ".norm.bias"))
-        Cc = sd[a + ".q.weight"].shape[0]
-        wq = torch.cat([sd[a + ".q.weight"], sd[a + ".k.weight"], sd[a + ".v.weight"]], 0).reshape(3 * Cc, Cc)
-        bq = torch.cat([sd[a + ".q.bias"], sd[a + ".k.bias"], sd[a + ".v.bias"]], 0)
-        E.attn.qkv = PackedConv(wq, bq, split=sp, device=dev)
-        E.attn.proj = PackedConv(sd[a + ".proj_out.weight"].reshape(Cc, Cc), sd[a + ".proj_out.bias"], split=sp, device=dev)
-        E.attn.C = Cc
+        E.attn = pk.attn_block("encoder.mid.attn_1")
         E.no_w, E.no_b = f32("encoder.norm_out.weight"), f32("encoder.norm_out.bias")
         E.conv_out = conv("encoder.conv_out")
         E.q_w = sd["quant_conv.weight"].float().reshape(sd["quant_conv.weight"].shape[0], -1).contiguous().to(dev)
         E.q_b = f32("quant_conv.bias")
         eres = [r for blk in E.down for r in blk.res] + [E.mid1, E.mid2]
-        E.stat_channels = (E.conv_in.cout + sum(2 * r.cout for r in eres) + E.attn.C
-                           + sum(blk.down.cout for blk in E.down if blk.down is not None))
+        E.stat_channels = blocks.stat_channels(E.conv_in, eres, [E.attn], [blk.down for blk in E.down])
         self.E = E
         self._epacked = True
 
@@ -420,34 +332,24 @@ class AutoencoderKL:
         R = NB * H * W
         x8 = torch.zeros(R, E.cin_pad, device=mel_rows.device, dtype=torch.float32)
         x8[:, :mel_rows.shape[1]] = mel_rows
-        xb = self._buf("a", (R, E.cin_pad * s), torch.bfloat16)
+        xb = self._bufs.get("a", (R, E.cin_pad * s), torch.bfloat16)
         L.cast_act(x8, NB, H, W, xb, split_off=E.cin_pad if sp else 0)
         ar = self._arena("enc", NB, E.stat_channels)
-        h = self._buf("econv_in", (R, E.conv_in.cout), torch.float32)
-        st = ar.slot("econv_in", NB, E.conv_in.cout)
-        run_conv(E.conv_in, xb, NB, H, W, out_f32=h, gn_stats=st, stats_hw=H * W)
+        bufs = self._bufs
+        h, st = blocks.conv_in(bufs, ar, "econv_in", E.conv_in, xb, NB, H, W)
         ch, cw = H, W
         for li, blk in enumerate(E.down):
             for bi, r in enumerate(blk.res):
-                h, st = self._resnet(f"edown{li}_{bi}", r, h, st, NB, ch, cw, ar)
+                h, st = blocks.resnet(bufs, ar, sp, f"edown{li}_{bi}", r, h, st, NB, ch, cw)
             if blk.down is not None:
-                Cc = blk.down.cin
-                xb = self._buf("a", (NB * ch * cw, Cc * s), torch.bfloat16)
-                L.cast_act(h, NB, ch, cw, xb, split_off=Cc if sp else 0)
-                hd = self._buf(f"edown{li}_ds", (NB * (ch // 2) * (cw // 2), blk.down.cout), torch.float32)
-                st = ar.slot(f"edown{li}_ds", NB, blk.down.cout)
-                run_conv(blk.down, xb, NB, ch, cw, out_f32=hd, gn_stats=st, stats_hw=(ch // 2) * (cw // 2))
+                h, st = blocks.downsample(bufs, ar, sp, f"edown{li}_ds", blk.down, h, NB, ch, cw)
                 ch, cw = ch // 2, cw // 2
-                h = hd
-        h, st = self._resnet("emid1", E.mid1, h, st, NB, ch, cw, ar)
+        h, st = blocks.resnet(bufs, ar, sp, "emid1", E.mid1, h, st, NB, ch, cw)
         h, st = self._attn(h, st, NB, ch, cw, ar, E.attn)
-        h, st = self._resnet("emid2", E.mid2, h, st, NB, ch, cw, ar)
-        Cc = h.shape[1]
-        a = self._buf("a", (NB * ch * cw, Cc * s), torch.bfloat16)
-        L.groupnorm(h, st, None, None, NB, ch * cw, 32, E.no_w, E.no_b, 1e-6, L.ACT_SILU, a, split_off=Cc if sp else 0)
-        mom = self._buf("emom", (NB * ch * cw, E.conv_out.cout), torch.float32)
-        run_conv(E.conv_out, a, NB, ch, cw, out_f32=mom)
-        out = self._buf("emoments", (NB * ch * cw, E.q_w.shape[0]), torch.float32)
+        h, st = blocks.resnet(bufs, ar, sp, "emid2", E.mid2, h, st, NB, ch, cw)
+        mom = bufs.get("emom", (NB * ch * cw, E.conv_out.cout), torch.float32)
+        blocks.norm_out(bufs, sp, h, st, NB, ch, cw, E.no_w, E.no_b, 1e-6, E.conv_out, mom)
+        out = self._bufs.get("emoments", (NB * ch * cw, E.q_w.shape[0]), torch.float32)
         L.linear_f32(mom, E.q_w, E.q_b, out)
         return out
 
@@ -470,31 +372,31 @@ class AutoencoderKL:
         self._pack()
         V, s, sp = self.V, self.s, self.split
         nm = mel_rows.shape[1]
-        xb = self._buf("hb", (B * T, nm * s), torch.bfloat16)
+        xb = self._bufs.get("hb", (B * T, nm * s), torch.bfloat16)
         L.cast_act(mel_rows, B, 1, T, xb, split_off=nm if sp else 0)
-        x = self._buf("hx_pre", (B * T, V.conv_pre.cout), torch.float32)
+        x = self._bufs.get("hx_pre", (B * T, V.conv_pre.cout), torch.float32)
         run_conv(V.conv_pre, xb, B, 1, T, out_f32=x)
         Lc = T
         for si, st in enumerate(V.stages):
-            xb = self._buf("hb", (B * Lc, st.cin * s), torch.bfloat16)
+            xb = self._bufs.get("hb", (B * Lc, st.cin * s), torch.bfloat16)
             L.cast_act(x, B, 1, Lc, xb, act=L.ACT_LRELU, act_param=0.1, split_off=st.cin if sp else 0)
-            Y = self._buf("hY", (B * Lc, st.k * st.cout), torch.float32)
+            Y = self._bufs.get("hY", (B * Lc, st.k * st.cout), torch.float32)
             run_conv(st.up, xb, B, 1, Lc, out_f32=Y)
             Lo = (Lc - 1) * st.u - 2 * st.pad + st.k
-            x = self._buf(f"hx{si}", (B * Lo, st.cout), torch.float32)
+            x = self._bufs.get(f"hx{si}", (B * Lo, st.cout), torch.float32)
             L.convt_gather(Y, B, Lc, st.k, st.cout, st.u, st.pad, Lo, st.up_bias, x)
             Lc = Lo
-            xs = self._buf(f"hxs{si}", (B * Lc, st.cout), torch.float32)
+            xs = self._bufs.get(f"hxs{si}", (B * Lc, st.cout), torch.float32)
             C_ = st.cout
             so = C_ if sp else 0
-            x_act = self._buf("hxa", (B * Lc, C_ * s), torch.bfloat16)  # lrelu(x): shared first operand of the 3 blocks
+            x_act = self._bufs.get("hxa", (B * Lc, C_ * s), torch.bfloat16)  # lrelu(x): shared first operand of the 3 blocks
             L.cast_act(x, B, 1, Lc, x_act, act=L.ACT_LRELU, act_param=0.1, split_off=so)
             nb = len(st.blocks)
             for j, rb in enumerate(st.blocks):
                 cur, cur_act = x, x_act
-                rbuf = self._buf("hrb", (B * Lc, C_), torch.float32)
-                ract = self._buf("hra", (B * Lc, C_ * s), torch.bfloat16)
-                xt = self._buf("hxt", (B * Lc, C_ * s), torch.bfloat16)
+                rbuf = self._bufs.get("hrb", (B * Lc, C_), torch.float32)
+                ract = self._bufs.get("hra", (B * Lc, C_ * s), torch.bfloat16)
+                xt = self._bufs.get("hxt", (B * Lc, C_ * s), torch.bfloat16)
                 nd = len(rb.c1)
                 for di in range(nd):
                     # xt = lrelu(conv1(lrelu(cur)))  (models.py:98-100), kept only as the bf16 operand of conv2
@@ -509,12 +411,12 @@ class AutoencoderKL:
                         run_conv(rb.c2[di], xt, B, 1, Lc, res=cur, alpha=1.0 / nb, accumulate=j > 0, out_f32=xs)
             x = xs
         cin = V.conv_post.cin
-        xb = self._buf("hb", (B * Lc, cin * s), torch.bfloat16)
+        xb = self._bufs.get("hb", (B * Lc, cin * s), torch.bfloat16)
         L.cast_act(x, B, 1, Lc, xb, act=L.ACT_LRELU, act_param=0.01, split_off=cin if sp else 0)  # F.leaky_relu default
-        y = self._buf("hpost", (B * Lc, 1), torch.float32)
+        y = self._bufs.get("hpost", (B * Lc, 1), torch.float32)
         run_conv(V.conv_post, xb, B, 1, Lc, out_f32=y)
-        wf = self._buf("hwave_f", (B, Lc), torch.float32)
-        wi = self._buf("hwave_i", (B, Lc), torch.int16)
+        wf = self._bufs.get("hwave_f", (B, Lc), torch.float32)
+        wi = self._bufs.get("hwave_i", (B, Lc), torch.int16)
         L.tanh_to_i16(y, B * Lc, 1, wf, wi)
         return wf, wi
 
