@@ -150,7 +150,6 @@ attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant
     // ---- online softmax (log2 domain); keys >= Lk score -inf
     const int kv0 = t * AT_BN;
     const bool tail = (kb != nullptr) || (kv0 + AT_BN > p.Lk);
-    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -162,46 +161,14 @@ attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant
         }
         s[4 * j + e] = fmaf(s[4 * j + e], sc, bias);
         s[4 * j + 2 + e] = fmaf(s[4 * j + 2 + e], sc, bias);
-        mx[0] = fmaxf(mx[0], s[4 * j + e]);
-        mx[1] = fmaxf(mx[1], s[4 * j + 2 + e]);
       }
     }
-    float corr[2], m_use[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-      const float m_new = fmaxf(m_run[h], mx[h]);
-      m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
-      corr[h] = ex2_approx(m_run[h] - m_use[h]);   // 0 on the first tile (m_run = -inf)
-      m_run[h] = m_new;
-      l_run[h] *= corr[h];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      o[4 * j] *= corr[0]; o[4 * j + 1] *= corr[0];
-      o[4 * j + 2] *= corr[1]; o[4 * j + 3] *= corr[1];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        s[4 * j + e] = ex2_approx(s[4 * j + e] - m_use[0]);
-        s[4 * j + 2 + e] = ex2_approx(s[4 * j + 2 + e] - m_use[1]);
-        l_run[0] += s[4 * j + e];
-        l_run[1] += s[4 * j + 2 + e];
-      }
-    }
-    // P as the A operand: k-step kk (keys [16kk, 16kk + 16)) = accumulator registers [8kk, 8kk + 8)
+    float corr[2];
+    softmax_step(s, m_run, l_run, corr);
+    rescale_rows(o, corr);
     uint32_t pa[NSPLIT][4][4];
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const float x0 = s[8 * kk + 2 * r], x1 = s[8 * kk + 2 * r + 1];
-        pa[0][kk][r] = pack_bf16(x0, x1);
-        if (NSPLIT == 2)
-          pa[NSPLIT - 1][kk][r] = pack_bf16(x0 - __bfloat162float(__float2bfloat16_rn(x0)),
-                                            x1 - __bfloat162float(__float2bfloat16_rn(x1)));
-      }
-    }
+    pack_p(pa[0], s);
+    if constexpr (NSPLIT == 2) pack_p<true>(pa[1], s);
 
     // ---- O += P V  (V rows = keys: MN-major B operand, 16 keys = 2048 bytes per k-step)
     mbar_wait(&full_v[buf], ph);
@@ -222,13 +189,7 @@ attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant
 
   // ---- finalize: O / l -> bf16 (hi/lo)
   float inv[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float l = l_run[h];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    inv[h] = 1.0f / l;
-  }
+  softmax_inv(l_run, inv);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int q = q0 + 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
@@ -239,8 +200,7 @@ attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant
       const float y0 = o[4 * j + 2 * h] * inv[h], y1 = o[4 * j + 2 * h + 1] * inv[h];
       *reinterpret_cast<uint32_t*>(op + 8 * j) = pack_bf16(y0, y1);
       if (p.split_off > 0)
-        *reinterpret_cast<uint32_t*>(op + p.split_off + 8 * j) =
-            pack_bf16(y0 - __bfloat162float(__float2bfloat16_rn(y0)), y1 - __bfloat162float(__float2bfloat16_rn(y1)));
+        *reinterpret_cast<uint32_t*>(op + p.split_off + 8 * j) = pack_bf16_lo(y0, y1);
     }
   }
 }
@@ -248,16 +208,10 @@ attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant
 template <int NSPLIT>
 static int launch_attn(const tng_attn_desc* d, const CUtensorMap& qm, const CUtensorMap& km, const CUtensorMap& vm,
                        const AttnParams& p, cudaStream_t st) {
-  using Cfg = AttnCfg<NSPLIT>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel<NSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error(TNG_ECUDA, "cudaFuncSetAttribute(attention): %s", cudaGetErrorString(e));
-    attr = true;
-  }
+  const int rc = set_max_dynamic_smem<attention_kernel<NSPLIT>>(AttnCfg<NSPLIT>::SMEM_BYTES, "attention");
+  if (rc) return rc;
   dim3 grid((d->Lq + AT_BM - 1) / AT_BM, d->heads, d->batch);
-  attention_kernel<NSPLIT><<<grid, AT_THREADS, Cfg::SMEM_BYTES, st>>>(qm, km, vm, p);
-  count_launch();
+  attention_kernel<NSPLIT><<<grid, AT_THREADS, AttnCfg<NSPLIT>::SMEM_BYTES, st>>>(qm, km, vm, p);
   return check_launch("attention");
 }
 
@@ -282,26 +236,10 @@ extern "C" int tng_attention(const tng_attn_desc* d, void* stream) {
   p.ld_o = d->ld_o; p.split_off = d->split_off;
   p.scale_log2e = d->scale * 1.4426950408889634f;
   CUtensorMap qm, km, vm;
-  uint32_t box[3] = {64, AT_BM, 1};
-  uint32_t kvbox[3] = {64, AT_BN, 1};
-  {
-    uint64_t dims[3] = {(uint64_t)d->ld_q, (uint64_t)d->Lq, (uint64_t)d->batch};
-    uint64_t str[2] = {(uint64_t)d->ld_q * 2, (uint64_t)d->ld_q * 2 * (uint64_t)d->Lq};
-    int rc = encode_tmap_bf16(&qm, d->q, 3, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)d->ld_k, (uint64_t)d->Lk, (uint64_t)d->batch};
-    uint64_t str[2] = {(uint64_t)d->ld_k * 2, (uint64_t)d->ld_k * 2 * (uint64_t)d->Lk};
-    int rc = encode_tmap_bf16(&km, d->k, 3, dims, str, kvbox);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)d->ld_v, (uint64_t)d->Lk, (uint64_t)d->batch};
-    uint64_t str[2] = {(uint64_t)d->ld_v * 2, (uint64_t)d->ld_v * 2 * (uint64_t)d->Lk};
-    int rc = encode_tmap_bf16(&vm, d->v, 3, dims, str, kvbox);
-    if (rc) return rc;
-  }
+  int rc = encode_tmap_rows_bf16(&qm, d->q, d->ld_q, d->Lq, d->batch, AT_BM);
+  if (!rc) rc = encode_tmap_rows_bf16(&km, d->k, d->ld_k, d->Lk, d->batch, AT_BN);
+  if (!rc) rc = encode_tmap_rows_bf16(&vm, d->v, d->ld_v, d->Lk, d->batch, AT_BN);
+  if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (d->nsplit == 2) return launch_attn<2>(d, qm, km, vm, p, st);
   return launch_attn<1>(d, qm, km, vm, p, st);

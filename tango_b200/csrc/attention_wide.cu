@@ -129,49 +129,14 @@ attention_wide_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_con
     }
 
     // ---- online softmax (log2 domain)
-    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        s[4 * j + e] *= sc;
-        s[4 * j + 2 + e] *= sc;
-        mx[0] = fmaxf(mx[0], s[4 * j + e]);
-        mx[1] = fmaxf(mx[1], s[4 * j + 2 + e]);
-      }
-    }
+    for (int i = 0; i < 32; ++i) s[i] *= sc;
     float corr[2];
+    softmax_step(s, m_run, l_run, corr);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-      const float m_new = fmaxf(m_run[h], mx[h]);
-      corr[h] = ex2_approx(m_run[h] - m_new);   // 0 on the first sub-tile (m_run = -inf)
-      m_run[h] = m_new;
-      l_run[h] *= corr[h];
-    }
-#pragma unroll
-    for (int n = 0; n < AW_DV / 64; ++n)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        o[n][4 * j] *= corr[0]; o[n][4 * j + 1] *= corr[0];
-        o[n][4 * j + 2] *= corr[1]; o[n][4 * j + 3] *= corr[1];
-      }
+    for (int n = 0; n < AW_DV / 64; ++n) rescale_rows(o[n], corr);
     uint32_t pa[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        s[4 * j + e] = ex2_approx(s[4 * j + e] - m_run[0]);
-        s[4 * j + 2 + e] = ex2_approx(s[4 * j + 2 + e] - m_run[1]);
-        l_run[0] += s[4 * j + e];
-        l_run[1] += s[4 * j + 2 + e];
-      }
-    }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-      for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+    pack_p(pa, s);
 
     // ---- O (+)= P_g V_g: 16 keys per k-step (16 x 128 B rows of each 64-column V chunk)
     mbar_wait(full_v, ph);
@@ -197,19 +162,18 @@ attention_wide_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_con
 
   // ---- finalize: O / l -> bf16
   const int t4 = lane & 3;
+  float inv[2];
+  softmax_inv(l_run, inv);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    float l = l_run[h];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv = 1.0f / l;
     const int q = q0 + 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
     __nv_bfloat16* op = p.out + (static_cast<long long>(b) * p.L + q) * p.ld_o + half * AW_DV + 2 * t4;
 #pragma unroll
     for (int n = 0; n < AW_DV / 64; ++n)
 #pragma unroll
       for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint32_t*>(op + 64 * n + 8 * j) = pack_bf16(o[n][4 * j + 2 * h] * inv, o[n][4 * j + 2 * h + 1] * inv);
+        *reinterpret_cast<uint32_t*>(op + 64 * n + 8 * j) =
+            pack_bf16(o[n][4 * j + 2 * h] * inv[h], o[n][4 * j + 2 * h + 1] * inv[h]);
   }
 }
 
@@ -231,35 +195,12 @@ extern "C" int tng_attention_wide(const void* q, int64_t ld_q, int32_t q_col0, c
   p.ld_o = ld_o;
   p.scale_log2e = scale * 1.4426950408889634f;
   CUtensorMap qm, km, vm;
-  {
-    uint64_t dims[3] = {(uint64_t)ld_q, (uint64_t)L, (uint64_t)batch};
-    uint64_t str[2] = {(uint64_t)ld_q * 2, (uint64_t)ld_q * 2 * (uint64_t)L};
-    uint32_t box[3] = {64, AW_BM, 1};
-    int rc = encode_tmap_bf16(&qm, q, 3, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)ld_k, (uint64_t)L, (uint64_t)batch};
-    uint64_t str[2] = {(uint64_t)ld_k * 2, (uint64_t)ld_k * 2 * (uint64_t)L};
-    uint32_t box[3] = {64, AW_SUB, 1};
-    int rc = encode_tmap_bf16(&km, k, 3, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)ld_v, (uint64_t)L, (uint64_t)batch};
-    uint64_t str[2] = {(uint64_t)ld_v * 2, (uint64_t)ld_v * 2 * (uint64_t)L};
-    uint32_t box[3] = {64, AW_SUB, 1};
-    int rc = encode_tmap_bf16(&vm, v, 3, dims, str, box);
-    if (rc) return rc;
-  }
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(attention_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM);
-    if (e != cudaSuccess) return set_error(TNG_ECUDA, "cudaFuncSetAttribute(attention_wide): %s", cudaGetErrorString(e));
-    attr = true;
-  }
+  int rc = encode_tmap_rows_bf16(&qm, q, ld_q, L, batch, AW_BM);
+  if (!rc) rc = encode_tmap_rows_bf16(&km, k, ld_k, L, batch, AW_SUB);
+  if (!rc) rc = encode_tmap_rows_bf16(&vm, v, ld_v, L, batch, AW_SUB);
+  if (!rc) rc = set_max_dynamic_smem<attention_wide_kernel>(AW_SMEM, "attention_wide");
+  if (rc) return rc;
   dim3 grid(L / AW_BM, AW_D / AW_DV, batch);
   attention_wide_kernel<<<grid, AW_THREADS, AW_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(qm, km, vm, p);
-  count_launch();
   return check_launch("attention_wide");
 }

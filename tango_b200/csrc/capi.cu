@@ -75,6 +75,13 @@ int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t
   return TNG_OK;
 }
 
+int encode_tmap_rows_bf16(CUtensorMap* out, const void* ptr, long long ld, long long L, long long batch, uint32_t rows) {
+  const uint64_t dims[3] = {(uint64_t)ld, (uint64_t)L, (uint64_t)batch};
+  const uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * (uint64_t)L};
+  const uint32_t box[3] = {64, rows, 1};
+  return encode_tmap_bf16(out, ptr, 3, dims, strides, box);
+}
+
 }  // namespace tng
 
 extern "C" int tng_version(void) { return 100; }

@@ -7,40 +7,6 @@
 
 namespace tng {
 
-__device__ __forceinline__ float4 load4(const void* base, int dt, long long idx) {
-  if (dt == TNG_DT_F32) return *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(base) + idx);
-  const uint2 u = *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(base) + idx);
-  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ void store4_bf16(__nv_bfloat16* p, float4 v) {
-  uint2 u;
-  u.x = pack_bf16(v.x, v.y);
-  u.y = pack_bf16(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = u;
-}
-__device__ __forceinline__ float bf16_lo(float v) { return v - __bfloat162float(__float2bfloat16_rn(v)); }
-__device__ __forceinline__ void store4_split(__nv_bfloat16* p, float4 v, int split_off) {
-  store4_bf16(p, v);
-  if (split_off > 0) store4_bf16(p + split_off, make_float4(bf16_lo(v.x), bf16_lo(v.y), bf16_lo(v.z), bf16_lo(v.w)));
-}
-__device__ __forceinline__ float act_f(float x, int act, float p) {
-  if (act == TNG_ACT_SILU) return silu_f(x);
-  if (act == TNG_ACT_LRELU) return x > 0.f ? x : x * p;
-  return x;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------------ GroupNorm
 // Thread layout: a CTA owns GN_ROWS pixels of one image; thread t keeps a FIXED channel quad q = t % QT and walks the
 // rows r = t / QT, + RL, ... (QT = min(C/4, 256) quad threads, RL = 256 / QT row lanes), so consecutive threads read
@@ -49,13 +15,8 @@ constexpr int GN_ROWS_MAX = 128;  // pixels per CTA (upper bound; the host shrin
 
 template <bool BF>
 __device__ __forceinline__ float4 ld_quad(const void* base, long long idx) {
-  if (BF) {
-    const uint2 u = *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(base) + idx);
-    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-    return make_float4(a.x, a.y, b.x, b.y);
-  }
-  return *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(base) + idx);
+  return BF ? load_bf16x4(static_cast<const __nv_bfloat16*>(base) + idx)
+            : *reinterpret_cast<const float4*>(static_cast<const float*>(base) + idx);
 }
 
 template <bool BF>
@@ -131,11 +92,11 @@ __device__ __forceinline__ void gn_apply_rows(const void* base, long long idx0, 
       if (SILU) { o.x = silu_f(o.x); o.y = silu_f(o.y); o.z = silu_f(o.z); o.w = silu_f(o.w); }
       __nv_bfloat16* yp = y + u * ystep;
       store4_bf16(yp, o);
-      if (SPLIT) store4_bf16(yp + split_off, make_float4(bf16_lo(o.x), bf16_lo(o.y), bf16_lo(o.z), bf16_lo(o.w)));
+      if (SPLIT) store4_bf16_lo(yp + split_off, o);
       if (RAW) {
         __nv_bfloat16* rp = raw + u * rstep;
         store4_bf16(rp, v[u]);
-        if (SPLIT) store4_bf16(rp + raw_split_off, make_float4(bf16_lo(v[u].x), bf16_lo(v[u].y), bf16_lo(v[u].z), bf16_lo(v[u].w)));
+        if (SPLIT) store4_bf16_lo(rp + raw_split_off, v[u]);
       }
     }
     if (RAW) raw += per * rstep;
@@ -370,14 +331,8 @@ __global__ void __launch_bounds__(128) rel_attention_kernel(const float* qkv, lo
     if (q >= L) break;
     const float inv = 1.0f / l[i];
     __nv_bfloat16* op = out + (static_cast<long long>(b) * L + q) * ld_o + h * 64;
-    const float y0 = o0[i] * inv, y1 = o1[i] * inv;
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(y0), h1 = __float2bfloat16_rn(y1);
-    op[lane] = h0;
-    op[lane + 32] = h1;
-    if (split_off > 0) {
-      op[split_off + lane] = __float2bfloat16_rn(y0 - __bfloat162float(h0));
-      op[split_off + lane + 32] = __float2bfloat16_rn(y1 - __bfloat162float(h1));
-    }
+    store_bf16_split(op + lane, o0[i] * inv, split_off);
+    store_bf16_split(op + lane + 32, o1[i] * inv, split_off);
   }
 }
 
@@ -457,10 +412,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* x, int L
   __syncthreads();
   const float inv = 1.0f / bc;
   for (int i = threadIdx.x; i < L; i += blockDim.x) {
-    const float p = expf(xr[i] * scale - m) * inv;
-    const __nv_bfloat16 hi = __float2bfloat16_rn(p);
-    y[row * ld_y + i] = hi;
-    if (split_off > 0) y[row * ld_y + split_off + i] = __float2bfloat16_rn(p - __bfloat162float(hi));
+    store_bf16_split(y + row * ld_y + i, expf(xr[i] * scale - m) * inv, split_off);
   }
 }
 
@@ -520,16 +472,8 @@ __global__ void __launch_bounds__(256) sched_step_kernel(const float* mo, long l
     }
     if (prev) prev[nchw] = out;
     if (next_in) {
-      const __nv_bfloat16 hi = __float2bfloat16_rn(out);
-      const __nv_bfloat16 lo = __float2bfloat16_rn(out - __bfloat162float(hi));
-      const long long r0 = (b * HW + hw) * ld_in + c;
-      next_in[r0] = hi;
-      if (split_off > 0) next_in[r0 + split_off] = lo;
-      if (cfg) {
-        const long long r1 = ((B + b) * HW + hw) * ld_in + c;
-        next_in[r1] = hi;
-        if (split_off > 0) next_in[r1 + split_off] = lo;
-      }
+      store_bf16_split(next_in + (b * HW + hw) * ld_in + c, out, split_off);
+      if (cfg) store_bf16_split(next_in + ((B + b) * HW + hw) * ld_in + c, out, split_off);
     }
   }
 }
@@ -619,9 +563,8 @@ __global__ void __launch_bounds__(256) stft_frames_kernel(const float* y, long l
       else if (src >= T) src = 2 * (T - 1) - src;
       v = y[b * T + src];
     }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    hi[i] = h;
-    lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+    hi[i] = __float2bfloat16_rn(v);
+    lo[i] = __float2bfloat16_rn(bf16_lo(v));
   }
 }
 
@@ -639,11 +582,7 @@ __global__ void __launch_bounds__(256) stft_magnitude_kernel(const float* F, lon
     const float re = f[b], im = f[bins + b];
     const float m = sqrtf(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im)));
     e = fmaf(m, m, e);
-    if (op) {
-      const __nv_bfloat16 h = __float2bfloat16_rn(m);
-      op[row * ld_op + b] = h;
-      if (split_off > 0) op[row * ld_op + split_off + b] = __float2bfloat16_rn(m - __bfloat162float(h));
-    }
+    if (op) store_bf16_split(op + row * ld_op + b, m, split_off);
     if (log_mag) log_mag[row * bins + b] = logf(fmaxf(m, floor_v));
   }
   e = warp_sum(e);
@@ -704,8 +643,43 @@ int launch_col_stats(const void* x, int dt, long long C, long long ld, long long
   const int gn_rows = gn_rows_for(NB, HW);
   dim3 grid((unsigned)((HW + gn_rows - 1) / gn_rows), (unsigned)NB);
   col_stats_kernel<<<grid, 256, 0, st>>>(x, dt, (int)C, ld, HW, col_stats, gn_rows);
-  count_launch();
   return check_launch("col_stats");
+}
+
+// One wave: the pixel blocks per (image, slab) are sized so that the grid fits the CTAs this instantiation can keep
+// resident (registers: 3 per SM for the plain variants), instead of leaving a partial second wave.
+template <bool SILU, bool SPLIT, bool RAW>
+static int launch_gn_apply(const void* x0, int dt0, int C0, const double* stats0, const void* x1, int dt1, int C1,
+                           const double* stats1, long long NB, long long HW, int nslabs, int groups, int tpg, int slab,
+                           const float* gamma, const float* beta, float eps, __nv_bfloat16* y, long long ld_y,
+                           int split_off, __nv_bfloat16* raw, long long ld_raw, int raw_split_off, cudaStream_t st) {
+  static int per_sm = 0;
+  if (per_sm == 0) {
+    int v = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, gn_apply_kernel<SILU, SPLIT, RAW>, 256, 0) != cudaSuccess || v < 1)
+      v = 2;
+    per_sm = v;
+  }
+  const int gn_rows = gn_rows_one_wave(NB * nslabs, HW, per_sm);
+  dim3 grid((unsigned)((HW + gn_rows - 1) / gn_rows), (unsigned)NB, (unsigned)nslabs);
+  gn_apply_kernel<SILU, SPLIT, RAW><<<grid, 256, 0, st>>>(x0, dt0, C0, stats0, x1, dt1, C1, stats1, HW, groups, tpg, slab,
+                                                          gamma, beta, eps, y, ld_y, split_off, raw, ld_raw, raw_split_off,
+                                                          gn_rows);
+  return check_launch("gn_apply");
+}
+
+// LayerNorm (RMS = false) and RMSNorm: the smallest NI that caches a row of C channels
+template <bool RMS>
+static int launch_layernorm(const float* x, long long rows, long long C, const float* gamma, const float* beta, float eps,
+                            void* y, long long ld_y, int split_off, float* y_f32, cudaStream_t st) {
+  const int wpb = 8;
+  const int ni = (int)((C / 4 + 31) / 32);
+  const auto kernel = ni <= 1 ? layernorm_kernel<1, RMS> : ni <= 2 ? layernorm_kernel<2, RMS>
+                    : ni <= 3 ? layernorm_kernel<3, RMS> : ni <= 5 ? layernorm_kernel<5, RMS>
+                    : ni <= 10 ? layernorm_kernel<10, RMS> : layernorm_kernel<16, RMS>;
+  kernel<<<ln_grid(rows, wpb), wpb * 32, 0, st>>>(x, rows, (int)C, gamma, beta, eps, reinterpret_cast<__nv_bfloat16*>(y),
+                                                  ld_y, split_off, y_f32);
+  return check_launch(RMS ? "rmsnorm" : "layernorm");
 }
 }  // namespace tng
 
@@ -732,73 +706,28 @@ extern "C" int tng_groupnorm_apply(const void* x0, int32_t dt0, int64_t C0, cons
   const int slab = gps * cpg, nslabs = groups / gps;
   int tpg = 1;
   while (tpg * 2 * gps <= 256 && tpg < 32) tpg *= 2;
-  const bool silu = act == TNG_ACT_SILU, split = split_off > 0, hasraw = raw_bf16 != nullptr;
-  // One wave: the pixel blocks per (image, slab) are sized so that the grid fits the CTAs this instantiation can keep
-  // resident (registers: 3 per SM for the plain variants), instead of leaving a partial second wave.
-#define TNG_GN_LAUNCH(S, P, R)                                                                                           \
-  do {                                                                                                                   \
-    static int per_sm = 0;                                                                                               \
-    if (per_sm == 0) {                                                                                                   \
-      int v = 0;                                                                                                         \
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, gn_apply_kernel<S, P, R>, 256, 0) != cudaSuccess || v < 1)   \
-        v = 2;                                                                                                           \
-      per_sm = v;                                                                                                        \
-    }                                                                                                                    \
-    const int gn_rows = gn_rows_one_wave(NB * nslabs, HW, per_sm);                                                       \
-    dim3 grid((unsigned)((HW + gn_rows - 1) / gn_rows), (unsigned)NB, (unsigned)nslabs);                                 \
-    gn_apply_kernel<S, P, R><<<grid, 256, 0, ST(stream)>>>(x0, dt0, (int)C0, stats0, x1, dt1, x1 ? (int)C1 : 0, stats1,  \
-                                                            HW, groups, tpg, slab, gamma, beta, eps,                     \
-                                                            reinterpret_cast<__nv_bfloat16*>(y), ld_y, split_off,        \
-                                                            reinterpret_cast<__nv_bfloat16*>(raw_bf16), ld_raw,          \
-                                                            raw_split_off, gn_rows);                                     \
-  } while (0)
-  if (silu) {
-    if (split) { if (hasraw) TNG_GN_LAUNCH(true, true, true); else TNG_GN_LAUNCH(true, true, false); }
-    else { if (hasraw) TNG_GN_LAUNCH(true, false, true); else TNG_GN_LAUNCH(true, false, false); }
-  } else {
-    if (split) { if (hasraw) TNG_GN_LAUNCH(false, true, true); else TNG_GN_LAUNCH(false, true, false); }
-    else { if (hasraw) TNG_GN_LAUNCH(false, false, true); else TNG_GN_LAUNCH(false, false, false); }
-  }
-#undef TNG_GN_LAUNCH
-  count_launch();
-  return check_launch("gn_apply");
+  using Launch = decltype(&launch_gn_apply<false, false, false>);
+  static constexpr Launch launch[2][2][2] = {   // [silu][hi/lo split][raw copy]
+      {{launch_gn_apply<false, false, false>, launch_gn_apply<false, false, true>},
+       {launch_gn_apply<false, true, false>, launch_gn_apply<false, true, true>}},
+      {{launch_gn_apply<true, false, false>, launch_gn_apply<true, false, true>},
+       {launch_gn_apply<true, true, false>, launch_gn_apply<true, true, true>}}};
+  return launch[act == TNG_ACT_SILU][split_off > 0][raw_bf16 != nullptr](
+      x0, dt0, (int)C0, stats0, x1, dt1, x1 ? (int)C1 : 0, stats1, NB, HW, nslabs, groups, tpg, slab, gamma, beta, eps,
+      reinterpret_cast<__nv_bfloat16*>(y), ld_y, split_off, reinterpret_cast<__nv_bfloat16*>(raw_bf16), ld_raw,
+      raw_split_off, ST(stream));
 }
 
 extern "C" int tng_layernorm(const float* x, int64_t rows, int64_t C, const float* gamma, const float* beta, float eps,
                              void* y, int64_t ld_y, int32_t split_off, void* stream) {
   if (!x || !y || !gamma || !beta || C % 4 || C > 2048 || ld_y % 4 || split_off % 4) return set_error(TNG_EINVAL, "layernorm: C=%lld unsupported", (long long)C);
-  const int wpb = 8;
-  const unsigned grid = ln_grid(rows, wpb);
-  const int ni = (int)((C / 4 + 31) / 32);
-#define TNG_LN(NI) layernorm_kernel<NI, false><<<grid, wpb * 32, 0, ST(stream)>>>(x, rows, (int)C, gamma, beta, eps, reinterpret_cast<__nv_bfloat16*>(y), ld_y, split_off, nullptr)
-  if (ni <= 1) TNG_LN(1);
-  else if (ni <= 2) TNG_LN(2);
-  else if (ni <= 3) TNG_LN(3);
-  else if (ni <= 5) TNG_LN(5);
-  else if (ni <= 10) TNG_LN(10);
-  else TNG_LN(16);
-#undef TNG_LN
-  count_launch();
-  return check_launch("layernorm");
+  return launch_layernorm<false>(x, rows, C, gamma, beta, eps, y, ld_y, split_off, nullptr, ST(stream));
 }
 
 extern "C" int tng_rmsnorm(const float* x, int64_t rows, int64_t C, const float* gamma, float eps, void* y, int64_t ld_y,
                            int32_t split_off, float* y_f32, void* stream) {
   if (!x || (!y && !y_f32) || !gamma || C % 4 || C > 2048 || ld_y % 4 || split_off % 4) return set_error(TNG_EINVAL, "rmsnorm: C=%lld unsupported", (long long)C);
-  const int wpb = 8;
-  const unsigned grid = ln_grid(rows, wpb);
-  const int ni = (int)((C / 4 + 31) / 32);
-  const float* beta = nullptr;
-#define TNG_RMS(NI) layernorm_kernel<NI, true><<<grid, wpb * 32, 0, ST(stream)>>>(x, rows, (int)C, gamma, beta, eps, reinterpret_cast<__nv_bfloat16*>(y), ld_y, split_off, y_f32)
-  if (ni <= 1) TNG_RMS(1);
-  else if (ni <= 2) TNG_RMS(2);
-  else if (ni <= 3) TNG_RMS(3);
-  else if (ni <= 5) TNG_RMS(5);
-  else if (ni <= 10) TNG_RMS(10);
-  else TNG_RMS(16);
-#undef TNG_RMS
-  count_launch();
-  return check_launch("rmsnorm");
+  return launch_layernorm<true>(x, rows, C, gamma, nullptr, eps, y, ld_y, split_off, y_f32, ST(stream));
 }
 
 extern "C" int tng_gather_rows(const float* table, int64_t n_table_rows, const int64_t* ids, int64_t rows, int64_t C,
@@ -809,7 +738,6 @@ extern "C" int tng_gather_rows(const float* table, int64_t n_table_rows, const i
   const int wpb = 8;
   gather_rows_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, ST(stream)>>>(
       table, reinterpret_cast<const long long*>(ids), rows, (int)C, out);
-  count_launch();
   return check_launch("gather_rows");
 }
 
@@ -820,7 +748,6 @@ extern "C" int tng_rel_attention(const float* qkv, int64_t ld, int32_t q_col0, i
   dim3 grid((unsigned)(batch * heads), (unsigned)((L + RA_QPB - 1) / RA_QPB));
   rel_attention_kernel<<<grid, 128, 0, ST(stream)>>>(qkv, ld, q_col0, k_col0, v_col0, heads, L, relbias, kbias,
                                                       reinterpret_cast<__nv_bfloat16*>(out), ld_o, split_off);
-  count_launch();
   return check_launch("rel_attention");
 }
 
@@ -831,7 +758,6 @@ extern "C" int tng_cast_act(const float* x, int64_t NB, int64_t H, int64_t W, in
   const long long total = NB * H * W * (upsample2x ? 4 : 1) * (C / 4);
   cast_act_kernel<<<grid_for(total), 256, 0, ST(stream)>>>(x, NB, (int)H, (int)W, (int)C, ld_x, upsample2x, act, act_param,
                                                             reinterpret_cast<__nv_bfloat16*>(y), ld_y, split_off);
-  count_launch();
   return check_launch("cast_act");
 }
 
@@ -840,7 +766,6 @@ extern "C" int tng_softmax_rows(const float* x, int64_t rows, int64_t L, int64_t
   if (!x || !y || rows <= 0 || L <= 0) return set_error(TNG_EINVAL, "softmax_rows: bad shape");
   softmax_rows_kernel<<<(unsigned)rows, 256, 0, ST(stream)>>>(x, (int)L, ld_x, scale, reinterpret_cast<__nv_bfloat16*>(y),
                                                                ld_y, split_off);
-  count_launch();
   return check_launch("softmax_rows");
 }
 
@@ -850,7 +775,6 @@ extern "C" int tng_transpose_bf16(const void* x, int64_t B, int64_t R, int64_t C
   dim3 grid((unsigned)((C + 31) / 32), (unsigned)((R + 31) / 32), (unsigned)B);
   transpose_bf16_kernel<<<grid, 256, 0, ST(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(x), (int)R, (int)C, ld_x,
                                                        reinterpret_cast<__nv_bfloat16*>(y), ld_y);
-  count_launch();
   return check_launch("transpose");
 }
 
@@ -861,7 +785,6 @@ extern "C" int tng_sched_step(const float* model_out, int64_t ld_mo, int32_t cfg
   sched_step_kernel<<<grid_for(B * C * HW), 256, 0, ST(stream)>>>(model_out, ld_mo, cfg, guidance, sample, noise, coef, prev,
                                                                   reinterpret_cast<__nv_bfloat16*>(next_in), ld_in,
                                                                   split_off, B, (int)C, HW);
-  count_launch();
   return check_launch("sched_step");
 }
 
@@ -869,7 +792,6 @@ extern "C" int tng_timestep_embedding(const float* t, int64_t n, int32_t dim, in
                                       float* out, void* stream) {
   if (!t || !out || dim < 2) return set_error(TNG_EINVAL, "timestep_embedding: bad argument");
   timestep_embedding_kernel<<<grid_for(n * (dim / 2)), 256, 0, ST(stream)>>>(t, n, dim, flip_sin_to_cos, freq_shift, out);
-  count_launch();
   return check_launch("timestep_embedding");
 }
 
@@ -878,7 +800,6 @@ extern "C" int tng_linear_f32(const float* x, int64_t M, int64_t K, const float*
   if (!x || !w || !y) return set_error(TNG_EINVAL, "linear_f32: null");
   const long long threads = M * N * 32;
   linear_f32_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, ST(stream)>>>(x, M, (int)K, w, b, (int)N, pre_act, post_act, y);
-  count_launch();
   return check_launch("linear_f32");
 }
 
@@ -887,14 +808,12 @@ extern "C" int tng_convt_gather(const float* Y, int64_t B, int64_t Lin, int32_t 
   if (!Y || !y || Cout % 4) return set_error(TNG_EINVAL, "convt_gather: bad shape");
   convt_gather_kernel<<<grid_for(B * Lout * (Cout / 4)), 256, 0, ST(stream)>>>(Y, B, Lin, ktaps, (int)Cout, stride, pad, Lout,
                                                                                bias, y);
-  count_launch();
   return check_launch("convt_gather");
 }
 
 extern "C" int tng_tanh_to_i16(const float* x, int64_t n, int64_t ld_x, float* wave_f32, int16_t* wave_i16, void* stream) {
   if (!x) return set_error(TNG_EINVAL, "tanh_to_i16: null");
   tanh_to_i16_kernel<<<grid_for(n), 256, 0, ST(stream)>>>(x, n, ld_x, wave_f32, wave_i16);
-  count_launch();
   return check_launch("tanh_to_i16");
 }
 
@@ -904,7 +823,6 @@ extern "C" int tng_stft_frames(const float* y, int64_t B, int64_t T, int32_t pad
     return set_error(TNG_EINVAL, "stft_frames: bad argument (reflect padding needs T > pad)");
   stft_frames_kernel<<<grid_for(B * ld), 256, 0, ST(stream)>>>(y, B, T, pad, reinterpret_cast<__nv_bfloat16*>(hi),
                                                                 reinterpret_cast<__nv_bfloat16*>(lo), ld);
-  count_launch();
   return check_launch("stft_frames");
 }
 
@@ -914,13 +832,11 @@ extern "C" int tng_stft_magnitude(const float* F, int64_t rows, int32_t bins, in
   const int wpb = 8;
   stft_magnitude_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, ST(stream)>>>(
       F, rows, bins, ldF, reinterpret_cast<__nv_bfloat16*>(mag_op), ld_op, split_off, log_mag, energy, floor_v);
-  count_launch();
   return check_launch("stft_magnitude");
 }
 
 extern "C" int tng_log_clamp(const float* x, int64_t n, float floor_v, float* y, void* stream) {
   if (!x || !y || n <= 0) return set_error(TNG_EINVAL, "log_clamp: bad argument");
   log_clamp_kernel<<<grid_for(n), 256, 0, ST(stream)>>>(x, n, floor_v, y);
-  count_launch();
   return check_launch("log_clamp");
 }

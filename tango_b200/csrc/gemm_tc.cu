@@ -73,12 +73,6 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 /*barriers*/;
 };
 
-__device__ __forceinline__ float apply_act(float x, int act, float p) {
-  if (act == TNG_ACT_SILU) return silu_f(x);
-  if (act == TNG_ACT_LRELU) return x > 0.f ? x : x * p;
-  return x;
-}
-
 struct EpiRows {
   long long row[ES];
   int img[ES];
@@ -103,14 +97,8 @@ __device__ __forceinline__ void epi_chunk(const GemmKernelParams& p, const float
       float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
       if (col_ok && ((R.valid >> i) & 1)) {
         if (VEC) {
-          if (p.res_bf16) {
-            const uint2 u = *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + R.row[i] * p.ldr + col);
-            const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-            const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-            r4 = make_float4(f0.x, f0.y, f1.x, f1.y);
-          } else {
-            r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + R.row[i] * p.ldr + col);
-          }
+          if (p.res_bf16) r4 = load_bf16x4(reinterpret_cast<const __nv_bfloat16*>(p.res) + R.row[i] * p.ldr + col);
+          else r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + R.row[i] * p.ldr + col);
         } else {
           float t[4] = {0.f, 0.f, 0.f, 0.f};
           for (int j = 0; j < 4; ++j)
@@ -186,27 +174,14 @@ __device__ __forceinline__ void epi_chunk(const GemmKernelParams& p, const float
     }
     if (has_bf) {
       __nv_bfloat16* op = p.out_bf16 + R.row[i] * p.ld_bf16 + col;
-      const float y0 = apply_act(a.x, p.act, p.act_param), y1 = apply_act(a.y, p.act, p.act_param);
-      const float y2 = apply_act(a.z, p.act, p.act_param), y3 = apply_act(a.w, p.act, p.act_param);
+      const float y0 = act_f(a.x, p.act, p.act_param), y1 = act_f(a.y, p.act, p.act_param);
+      const float y2 = act_f(a.z, p.act, p.act_param), y3 = act_f(a.w, p.act, p.act_param);
       if (VEC) {
-        uint2 u;
-        u.x = pack_bf16(y0, y1); u.y = pack_bf16(y2, y3);
-        *reinterpret_cast<uint2*>(op) = u;
-        if (p.split_off > 0) {
-          uint2 l;
-          l.x = pack_bf16(y0 - __bfloat162float(__float2bfloat16_rn(y0)), y1 - __bfloat162float(__float2bfloat16_rn(y1)));
-          l.y = pack_bf16(y2 - __bfloat162float(__float2bfloat16_rn(y2)), y3 - __bfloat162float(__float2bfloat16_rn(y3)));
-          *reinterpret_cast<uint2*>(op + p.split_off) = l;
-        }
+        store4_split(op, make_float4(y0, y1, y2, y3), p.split_off);
       } else {
         const float t[4] = {y0, y1, y2, y3};
-        for (int j = 0; j < 4; ++j) {
-          if (col + j < p.Ncols) {
-            const __nv_bfloat16 hi = __float2bfloat16_rn(t[j]);
-            op[j] = hi;
-            if (p.split_off > 0) op[p.split_off + j] = __float2bfloat16_rn(t[j] - __bfloat162float(hi));
-          }
-        }
+        for (int j = 0; j < 4; ++j)
+          if (col + j < p.Ncols) store_bf16_split(op + j, t[j], p.split_off);
       }
     }
   }
@@ -230,12 +205,7 @@ __device__ __forceinline__ void epi_chunk_full(const GemmKernelParams& p, const 
       const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + r0 * p.ldr + col;
       const long long rs = 4 * p.ldr;
 #pragma unroll
-      for (int i = 0; i < ES; ++i) {
-        const uint2 u = *reinterpret_cast<const uint2*>(rp + i * rs);
-        const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-        const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-        rres[i] = make_float4(f0.x, f0.y, f1.x, f1.y);
-      }
+      for (int i = 0; i < ES; ++i) rres[i] = load_bf16x4(rp + i * rs);
     } else {
       const float* rp = reinterpret_cast<const float*>(p.res) + r0 * p.ldr + col;
       const long long rs = 4 * p.ldr;
@@ -321,20 +291,11 @@ __device__ __forceinline__ void epi_chunk_full(const GemmKernelParams& p, const 
     __nv_bfloat16* op = p.out_bf16 + r0 * p.ld_bf16 + col;
     const long long os = 4 * p.ld_bf16;
 #pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      uint2 u;
-      u.x = pack_bf16(a[i].x, a[i].y); u.y = pack_bf16(a[i].z, a[i].w);
-      *reinterpret_cast<uint2*>(op + i * os) = u;
-    }
+    for (int i = 0; i < ES; ++i) store4_bf16(op + i * os, a[i]);
     if (p.split_off > 0) {
       op += p.split_off;
 #pragma unroll
-      for (int i = 0; i < ES; ++i) {
-        uint2 l;
-        l.x = pack_bf16(a[i].x - __bfloat162float(__float2bfloat16_rn(a[i].x)), a[i].y - __bfloat162float(__float2bfloat16_rn(a[i].y)));
-        l.y = pack_bf16(a[i].z - __bfloat162float(__float2bfloat16_rn(a[i].z)), a[i].w - __bfloat162float(__float2bfloat16_rn(a[i].w)));
-        *reinterpret_cast<uint2*>(op + i * os) = l;
-      }
+      for (int i = 0; i < ES; ++i) store4_bf16_lo(op + i * os, a[i]);
     }
   }
 }
@@ -416,10 +377,8 @@ __device__ __forceinline__ void epi_tile_splitk(const GemmKernelParams& p, float
         }
         if (p.res) {
           if (p.res_bf16) {
-            const uint2 u = *reinterpret_cast<const uint2*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + row * p.ldr + col);
-            const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-            const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-            a.x += f0.x; a.y += f0.y; a.z += f1.x; a.w += f1.y;
+            const float4 r4 = load_bf16x4(reinterpret_cast<const __nv_bfloat16*>(p.res) + row * p.ldr + col);
+            a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
           } else {
             const float4 r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + row * p.ldr + col);
             a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
@@ -481,10 +440,7 @@ __device__ __forceinline__ void epi_tile_geglu(const GemmKernelParams& p, float*
       *reinterpret_cast<uint2*>(op + i * os) = u;
       if (SPLIT) {
         uint2 l;
-        l.x = pack_bf16(hid[i].x - __bfloat162float(__float2bfloat16_rn(hid[i].x)),
-                        hid[i].y - __bfloat162float(__float2bfloat16_rn(hid[i].y)));
-        l.y = pack_bf16(hid[i].z - __bfloat162float(__float2bfloat16_rn(hid[i].z)),
-                        hid[i].w - __bfloat162float(__float2bfloat16_rn(hid[i].w)));
+        l.x = pack_bf16_lo(hid[i].x, hid[i].y); l.y = pack_bf16_lo(hid[i].z, hid[i].w);
         *reinterpret_cast<uint2*>(op + p.split_off + i * os) = l;
       }
     }
@@ -664,19 +620,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
 template <int BN>
 static int launch_gemm(const CUtensorMap* am, const CUtensorMap& bm, const GemmKernelParams& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error(TNG_ECUDA, "cudaFuncSetAttribute(gemm_tc<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
+  const int rc = set_max_dynamic_smem<gemm_tc_kernel<BN>>(Cfg::SMEM_BYTES, "gemm_tc");
+  if (rc) return rc;
   const int work = p.m_tiles * p.n_tiles * p.ksplit;
   const int grid = work < num_sms() ? work : num_sms();
   gemm_tc_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(am[0], am[1], am[2], am[3], bm, p);
-  count_launch();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(TNG_ECUDA, "gemm_tc<%d> launch: %s", BN, cudaGetErrorString(e));
-  return TNG_OK;
+  return check_launch("gemm_tc");
 }
 
 static bool is_pow2(long long x) { return x > 0 && (x & (x - 1)) == 0; }

@@ -1,12 +1,15 @@
-// tng_ptx.cuh — thin inline-PTX wrappers for sm_90a (Hopper H100):
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with shared-memory descriptors), fences.
-// Everything here is hand-written PTX; no CUTLASS / CuTe dependency.
+// tng_ptx.cuh — the device helpers shared by the kernels of libtango_b200.so (sm_90a, Hopper H100):
+//   * thin inline-PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with shared-memory
+//     descriptors), fences; hand-written PTX, no CUTLASS / CuTe dependency;
+//   * the flash-attention online-softmax step on a wgmma score fragment;
+//   * activations, warp / quad reductions, and bf16 I/O including the hi/lo split of the "split" precision.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda.h>
 #include <stdint.h>
 #include <stdio.h>
+#include "../../include/tango_b200.h"
 
 namespace tng {
 
@@ -25,9 +28,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
@@ -263,9 +263,129 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
   const float w = x * fmaf(x * x, 0.044715f, 1.0f);
   return x * rcp_approx(1.0f + ex2_approx(w * -2.3022081986f));   // 2 sqrt(2/pi) log2(e)
 }
+__device__ __forceinline__ float act_f(float x, int act, float p) {
+  if (act == TNG_ACT_SILU) return silu_f(x);
+  if (act == TNG_ACT_LRELU) return x > 0.f ? x : x * p;
+  return x;
+}
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+// over the four lanes that hold one row of a wgmma accumulator (lanes 4i .. 4i + 3)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+
+// ---------------------------------------------------------------- bf16 I/O
+// The "split" precision stores an operand x as hi = bf16_rn(x) and, split_off elements further, lo = bf16_rn(bf16_lo(x)).
+// The split GEMM and attention kernels rely on this exact residual; every writer of a lo half uses the helpers below.
+__device__ __forceinline__ float bf16_lo(float v) { return v - __bfloat162float(__float2bfloat16_rn(v)); }
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ uint32_t pack_bf16_lo(float a, float b) { return pack_bf16(bf16_lo(a), bf16_lo(b)); }
+__device__ __forceinline__ float4 load_bf16x4(const __nv_bfloat16* p) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
+  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ void store4_bf16(__nv_bfloat16* p, float4 v) {
+  uint2 u;
+  u.x = pack_bf16(v.x, v.y);
+  u.y = pack_bf16(v.z, v.w);
+  *reinterpret_cast<uint2*>(p) = u;
+}
+__device__ __forceinline__ void store4_bf16_lo(__nv_bfloat16* p, float4 v) {
+  store4_bf16(p, make_float4(bf16_lo(v.x), bf16_lo(v.y), bf16_lo(v.z), bf16_lo(v.w)));
+}
+// hi at p and, when split_off > 0, lo at p + split_off
+__device__ __forceinline__ void store4_split(__nv_bfloat16* p, float4 v, int split_off) {
+  store4_bf16(p, v);
+  if (split_off > 0) store4_bf16_lo(p + split_off, v);
+}
+__device__ __forceinline__ void store_bf16_split(__nv_bfloat16* p, float v, int split_off) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  *p = hi;
+  if (split_off > 0) p[split_off] = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+
+// ---------------------------------------------------------------- flash attention on wgmma fragments
+// A 64 x 64 score tile in the accumulator layout of a warpgroup (see wgmma above): this thread holds rows r and r + 8
+// of its warp's 16, s[4j + {0, 1}] of row r and s[4j + {2, 3}] of row r + 8. Index 0 / 1 of the per-row arrays below is
+// row r / r + 8; l_run is this lane's partial sum (the quad's lanes are combined by softmax_inv).
+//
+// One online-softmax step in the log2 domain: s holds the scaled scores (masked keys at -inf) and becomes the
+// unnormalised probabilities 2^(s - m); m_run / l_run are updated; corr receives the factor by which everything
+// accumulated over the previous tiles must be scaled. A row whose scores are all -inf so far keeps m_run = -inf and
+// gets probabilities 0 (instead of the NaN of -inf - -inf).
+__device__ __forceinline__ void softmax_step(float (&s)[32], float (&m_run)[2], float (&l_run)[2], float (&corr)[2]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      mx[0] = fmaxf(mx[0], s[4 * j + e]);
+      mx[1] = fmaxf(mx[1], s[4 * j + 2 + e]);
+    }
+  }
+  float m_use[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float m_new = fmaxf(m_run[h], quad_max(mx[h]));
+    m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
+    corr[h] = ex2_approx(m_run[h] - m_use[h]);   // 0 on the first tile (m_run = -inf)
+    m_run[h] = m_new;
+    l_run[h] *= corr[h];
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      s[4 * j + e] = ex2_approx(s[4 * j + e] - m_use[0]);
+      s[4 * j + 2 + e] = ex2_approx(s[4 * j + 2 + e] - m_use[1]);
+      l_run[0] += s[4 * j + e];
+      l_run[1] += s[4 * j + 2 + e];
+    }
+  }
+}
+// o: a [64 x 64] output accumulator in the same layout
+__device__ __forceinline__ void rescale_rows(float (&o)[32], const float (&corr)[2]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    o[4 * j] *= corr[0]; o[4 * j + 1] *= corr[0];
+    o[4 * j + 2] *= corr[1]; o[4 * j + 3] *= corr[1];
+  }
+}
+// P as the register A operand of O += P V: k-step kk (keys [16kk, 16kk + 16)) = accumulator registers [8kk, 8kk + 8).
+// LO packs the bf16 residuals instead (the lo half of P in the split precision).
+template <bool LO = false>
+__device__ __forceinline__ void pack_p(uint32_t (&pa)[4][4], const float (&s)[32]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const float x0 = s[8 * kk + 2 * r], x1 = s[8 * kk + 2 * r + 1];
+      pa[kk][r] = LO ? pack_bf16_lo(x0, x1) : pack_bf16(x0, x1);
+    }
+}
+// the final normalisation: 1 / (row sum) of both rows
+__device__ __forceinline__ void softmax_inv(const float (&l_run)[2], float (&inv)[2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) inv[h] = 1.0f / quad_sum(l_run[h]);
 }
 
 }  // namespace tng
