@@ -225,6 +225,29 @@ int tng_sched_step(const float* model_out, int64_t ld_mo, int32_t cfg, float gui
                    int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Fused classifier-free guidance + multistep DPM-Solver(++) update (one HBM pass).
+ * Replaces: models.py:244-249 and DPMSolverMultistepScheduler.step (scheduling_dpmsolver_multistep.py:429-495:
+ *           convert_model_output :243-281 and the order-1/2/3 updates :305-427).
+ * coef = float[11] {c_a, c_b, c_d, c_s, c_0, c_1, c_2, 1/r0, 1/r1, r0/(r0+r1), 1/(r0+r1)}: fp32 scalars computed on
+ *         the host with the reference's own fp32 op order, signs folded in (device pointer).
+ *   v    = u + guidance * (t - u)  (cfg) or the model output itself
+ *   m0   = (c_a * sample + c_b * v) / c_d                              written to the history slot m0
+ *   order 1: x = c_s * sample - c_0 * m0
+ *   order 2: x = (c_s * sample - c_0 * m0) + c_1 * D1,                D1 = (1/r0) * (m0 - m1)
+ *   order 3: x = ((c_s * sample - c_0 * m0) + c_1 * D1) - c_2 * D2,   D1_0 = (1/r0) * (m0 - m1),
+ *            D1_1 = (1/r1) * (m1 - m2), D1 = D1_0 + (r0/(r0+r1)) * (D1_0 - D1_1), D2 = (1/(r0+r1)) * (D1_0 - D1_1)
+ * every product / sum is one round-to-nearest fp32 op (no fma), so x equals the reference's CPU fp32 result bit
+ * for bit. model_out: fp32 channels-last [(2)B, HW, C] (uncond half first when cfg); sample, m0 / m1 / m2 (the
+ * converted outputs of this, the previous and the one-before step; m1 is needed for order >= 2, m2 for order 3)
+ * and prev: fp32 NCHW [B, C, HW]; prev may alias sample. The caller rotates the history slots. Also writes
+ * next_in: the channels-last bf16 UNet input [(2)B, HW, ld_in] (duplicated for the CFG halves, hi/lo split at
+ * split_off when > 0).
+ */
+int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
+                 const float* coef, int32_t order, float* m0, const float* m1, const float* m2, float* prev,
+                 void* next_in, int64_t ld_in, int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Small exact-fp32 pieces.
  * tng_timestep_embedding: get_timestep_embedding (embeddings.py:22-62), flip_sin_to_cos / freq_shift configurable.
  * tng_linear_f32: y = act(x) @ W^T + b for tiny M (TimestepEmbedding, resnet time_emb_proj; embeddings.py:200-212,

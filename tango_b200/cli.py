@@ -43,7 +43,10 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     p.add_argument("--output_root", type=str, default="outputs")
     p.add_argument("--exp_id", type=str, default=None, help="Run id (default: unix time; pass one under torchrun)")
     p.add_argument("--precision", default="bf16", choices=["bf16", "split"])
-    p.add_argument("--scheduler", default="ddpm", choices=["ddpm", "ddim"], help="inference_hf.py uses DDPM")
+    p.add_argument("--scheduler", default="ddpm", choices=["ddpm", "ddim", "dpmsolver++"],
+                   help="inference_hf.py uses DDPM; dpmsolver++ samples in 20-25 steps")
+    p.add_argument("--solver_order", type=int, default=2, choices=[1, 2, 3], help="DPM-Solver++ order (--scheduler "
+                   "dpmsolver++ only)")
     p.add_argument("--latent_h", type=int, default=256, help="latent frames: 256 = 10.24 s (reference)")
     p.add_argument("--seed", type=int, default=None, help="torch.manual_seed for reproducible noise")
     return p.parse_args(argv)
@@ -75,17 +78,22 @@ def output_dir_for(root: str, exp_id: str, num_steps: int, guidance: float) -> s
     return os.path.join(root, "{}_steps_{}_guidance_{}".format(exp_id, num_steps, guidance))
 
 
-def build_tango(checkpoint: str, device: str, precision: str, scheduler: str):
+def build_tango(checkpoint: str, device: str, precision: str, scheduler: str, solver_order: int = 2):
     from . import synth
     from .pipeline import Tango
     if checkpoint.startswith("synthetic"):
         kind = checkpoint.split(":", 1)[1] if ":" in checkpoint else "base"
         ucfg = {"tiny": synth.TINY_UNET_CONFIG, "base": synth.BASE_UNET_CONFIG, "xl": synth.XL_UNET_CONFIG}[kind]
-        return Tango.from_synthetic(ucfg, device=device, precision=precision, scheduler=scheduler)
-    t = Tango(checkpoint, device, precision=precision)
-    if scheduler == "ddim":
-        from .schedulers import DDIMScheduler
-        t.scheduler = DDIMScheduler.from_pretrained(t.scheduler_name, subfolder="scheduler")   # same scheduler_config.json
+        t = Tango.from_synthetic(ucfg, device=device, precision=precision, scheduler=scheduler)
+    else:
+        t = Tango(checkpoint, device, precision=precision)
+        if scheduler == "ddim":
+            from .schedulers import DDIMScheduler
+            t.scheduler = DDIMScheduler.from_pretrained(t.scheduler_name, subfolder="scheduler")   # same scheduler_config.json
+    if scheduler == "dpmsolver++":
+        from .schedulers import DPMSolverMultistepScheduler
+        # the betas and prediction type of the checkpoint's scheduler_config.json, as diffusers' from_config does
+        t.scheduler = DPMSolverMultistepScheduler.from_config(t.scheduler.config, solver_order=solver_order)
     return t
 
 
@@ -117,7 +125,7 @@ def main(argv: Optional[Sequence[str]] = None) -> dict:
     out_dir = output_dir_for(args.output_root, exp_id, args.num_steps, args.guidance)
     os.makedirs(out_dir, exist_ok=True)
 
-    tango = build_tango(args.checkpoint, device, args.precision, args.scheduler)
+    tango = build_tango(args.checkpoint, device, args.precision, args.scheduler, args.solver_order)
     kw = {} if args.latent_h == 256 else {"latent_shape": (args.latent_h, 16)}
     torch.cuda.synchronize()
     t0 = time.time()

@@ -24,7 +24,7 @@ SYMBOLS = [
     "tng_groupnorm_stats", "tng_groupnorm_apply", "tng_layernorm", "tng_cast_act", "tng_softmax_rows",
     "tng_transpose_bf16", "tng_sched_step", "tng_timestep_embedding", "tng_linear_f32", "tng_convt_gather",
     "tng_tanh_to_i16", "tng_rmsnorm", "tng_gather_rows", "tng_rel_attention", "tng_stft_frames", "tng_stft_magnitude",
-    "tng_log_clamp", "tng_attention_wide", "tng_gemm_plan",
+    "tng_log_clamp", "tng_attention_wide", "tng_gemm_plan", "tng_dpm_step",
 ]
 
 
@@ -104,6 +104,7 @@ def load(build_if_missing: bool = True) -> C.CDLL:
         "tng_softmax_rows": [vp, i64, i64, i64, f32, vp, i64, i32, vp],
         "tng_transpose_bf16": [vp, i64, i64, i64, i64, vp, i64, vp],
         "tng_sched_step": [vp, i64, i32, f32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
+        "tng_dpm_step": [vp, i64, i32, f32, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
         "tng_timestep_embedding": [vp, i64, i32, i32, f32, vp, vp],
         "tng_linear_f32": [vp, i64, i64, vp, vp, i64, i32, i32, vp, vp],
         "tng_convt_gather": [vp, i64, i64, i32, i64, i32, i32, i64, vp, vp, vp],
@@ -390,6 +391,18 @@ def sched_step(model_out, cfg, guidance, sample, noise, coef, prev, next_in, *, 
         + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
     _call("sched_step", nbytes, load().tng_sched_step, ptr(model_out), 0 if model_out is None else model_out.stride(0),
           int(cfg), guidance, sample.data_ptr(), ptr(noise), coef.data_ptr(), ptr(prev), ptr(next_in),
+          0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
+
+
+def dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, next_in, *, B, Cc, HW, split_off=0):
+    """tng_dpm_step: CFG combine + DPM-Solver(++) update of `order` (1-3) from the history slots m0 (written) / m1 / m2
+    (read) + packing of the next UNet input; see include/tango_b200.h."""
+    require_cuda(model_out, sample, coef, m0, m1, m2, prev, next_in)
+    n = B * Cc * HW
+    nbytes = n * 4 * ((2 if cfg else 1) + 1 + 1 + (order - 1) + (prev is not None)) \
+        + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
+    _call("dpm_step", nbytes, load().tng_dpm_step, model_out.data_ptr(), model_out.stride(0), int(cfg), guidance,
+          sample.data_ptr(), coef.data_ptr(), order, m0.data_ptr(), ptr(m1), ptr(m2), ptr(prev), ptr(next_in),
           0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
 
 

@@ -1,9 +1,11 @@
-"""DDPM / DDIM schedulers with the reference's interface; the update itself runs in one fused CUDA kernel.
+"""DDPM / DDIM / multistep DPM-Solver schedulers with the reference's interface; the update itself runs in one fused
+CUDA kernel.
 
 Mirrors diffusers' DDPMScheduler / DDIMScheduler as Tango uses them
 (/root/reference/mustango/diffusers/src/diffusers/schedulers/scheduling_ddpm.py:122-349,
 scheduling_ddim.py:132-359; call sites models.py:224-249, tango.py:36): `set_timesteps`, `timesteps`,
-`init_noise_sigma`, `order`, `scale_model_input`, `step(...).prev_sample`, `config`.
+`init_noise_sigma`, `order`, `scale_model_input`, `step(...).prev_sample`, `config`. DPMSolverMultistepScheduler
+(scheduling_dpmsolver_multistep.py:57-535) is the opt-in few-step sampler; its update runs in tng_dpm_step (below).
 
 All per-step scalars are computed on the host with the reference's own fp32 torch ops (same association order),
 packed into a [num_steps, 10] coefficient table and shipped to the device once per `set_timesteps`; the kernel
@@ -85,7 +87,14 @@ class _SchedulerBase:
             raise ValueError(f"scheduler '{name}' is not reachable offline: pass a local directory holding its "
                              "scheduler_config.json (only stabilityai/stable-diffusion-2-1 is built in)")
         base.update(overrides)
-        return cls(**{k: v for k, v in base.items() if k in cls._ACCEPTED})
+        return cls.from_config(base)
+
+    @classmethod
+    def from_config(cls, config: dict, **overrides):
+        """diffusers' `from_config`: the keys this scheduler's constructor accepts are kept, the rest dropped, so
+        `DPMSolverMultistepScheduler.from_config(ddpm.config)` builds a DPM-Solver on the DDPM's betas."""
+        cfg = dict(config, **overrides)
+        return cls(**{k: v for k, v in cfg.items() if k in cls._ACCEPTED})
 
     def __len__(self):
         return self.config["num_train_timesteps"]
@@ -108,7 +117,7 @@ class _SchedulerBase:
         key = tuple(self._t_list)
         cache = self.__dict__.setdefault("_table_cache", {})
         if key not in cache:   # ~40 tiny fp32 torch ops per step: computed once per grid, reused by later calls
-            cache[key] = torch.stack([self._coefficients(t) for t in self._t_list]).contiguous()
+            cache[key] = torch.stack(self._table_rows()).contiguous()
         self._coef_host = cache[key]
         self._t_index = {t: i for i, t in enumerate(self._t_list)}
         self._coef_dev = None
@@ -116,6 +125,17 @@ class _SchedulerBase:
             self.timesteps = self.timesteps.to(device)
             if torch.device(device).type == "cuda":
                 self._coef_dev = self._coef_host.to(device)
+
+    def _table_rows(self) -> list:
+        """Row i of the coefficient table belongs to timesteps[i]."""
+        return [self._coefficients(t) for t in self._t_list]
+
+    def _loop_step(self, i: int, model_out, cfg: bool, guidance: float, sample, noise, coef, next_in, bufs, *, B, Cc,
+                   HW, split_off):
+        """Step i of AudioDiffusion.inference: one fused CFG + update + next-UNet-input launch, `sample` updated in
+        place. `bufs` holds the loop's persistent buffers of this shape."""
+        L.sched_step(model_out, cfg, guidance, sample, noise, coef[i], sample, next_in, B=B, Cc=Cc, HW=HW,
+                     split_off=split_off)
 
     def timestep_at(self, i: int) -> int:
         """Host copy of timesteps[i] (no device sync)."""
@@ -271,3 +291,192 @@ class DDIMScheduler(_SchedulerBase):
         clip = torch.tensor(float(cfg["clip_sample_range"]) if cfg["clip_sample"] else 0.0)
         return torch.stack([c_x0_s, c_x0_m, c_prev_x0, zero, zero, c_eps_s, c_eps_m, c_prev_eps, clip,
                             c_div]).float()
+
+
+NCOEF_DPM = 11
+
+
+class DPMSolverMultistepScheduler(_SchedulerBase):
+    """Multistep DPM-Solver / DPM-Solver++ (scheduling_dpmsolver_multistep.py:57-535), for sampling in 20-25 steps.
+
+    The CFG combine, `convert_model_output` and the order-1/2/3 update run as one tng_dpm_step launch. Its per-step
+    scalars are computed here with the reference's own fp32 torch ops in the reference's order and packed into a
+    [num_steps, 11] table (see include/tango_b200.h for the row): {c_a, c_b, c_d} convert the model output,
+    m0 = (c_a * sample + c_b * v) / c_d; {c_s, c_0, c_1, c_2} weigh sample, D0, D1 and D2; then 1/r0, 1/r1,
+    r0/(r0+r1) and 1/(r0+r1). Signs are folded into the coefficients, which IEEE arithmetic allows without changing a
+    bit (x - y*z == x + (-y)*z). Row i uses the order that step i takes in a loop started by `set_timesteps`
+    (`lower_order_nums` bookkeeping and the final-step rules, :464-490); `step` called out of that sequence gets a
+    row of its own. Dynamic thresholding (per-sample quantile; unsuitable for latent diffusion per the fork's own
+    docstring) is not implemented."""
+
+    _ACCEPTED = ("num_train_timesteps", "beta_start", "beta_end", "beta_schedule", "trained_betas", "solver_order",
+                 "prediction_type", "thresholding", "dynamic_thresholding_ratio", "sample_max_value", "algorithm_type",
+                 "solver_type", "lower_order_final")
+
+    def __init__(self, num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, beta_schedule="linear",
+                 trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                 dynamic_thresholding_ratio=0.995, sample_max_value=1.0, algorithm_type="dpmsolver++",
+                 solver_type="midpoint", lower_order_final=True):
+        if thresholding:
+            raise NotImplementedError("thresholding=True (dynamic thresholding) is not implemented for "
+                                      "DPMSolverMultistepScheduler: it is unsuitable for latent diffusion")
+        if algorithm_type == "deis":          # :166-170
+            algorithm_type = "dpmsolver++"
+        elif algorithm_type not in ("dpmsolver", "dpmsolver++"):
+            raise NotImplementedError(f"{algorithm_type} does is not implemented for {self.__class__}")
+        if solver_type in ("logrho", "bh1", "bh2"):   # :172-176
+            solver_type = "midpoint"
+        elif solver_type not in ("midpoint", "heun"):
+            raise NotImplementedError(f"{solver_type} does is not implemented for {self.__class__}")
+        if solver_order not in (1, 2, 3):
+            raise ValueError(f"solver_order must be 1, 2 or 3, got {solver_order}")
+        if prediction_type not in ("epsilon", "sample", "v_prediction"):
+            raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample`, or"
+                             " `v_prediction` for the DPMSolverMultistepScheduler.")
+        super().__init__(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                         beta_schedule=beta_schedule, trained_betas=trained_betas, solver_order=solver_order,
+                         prediction_type=prediction_type, thresholding=thresholding,
+                         dynamic_thresholding_ratio=dynamic_thresholding_ratio, sample_max_value=sample_max_value,
+                         algorithm_type=algorithm_type, solver_type=solver_type, lower_order_final=lower_order_final)
+        # :157-160, VP-type noise schedule
+        self.alpha_t = torch.sqrt(self.alphas_cumprod)
+        self.sigma_t = torch.sqrt(1 - self.alphas_cumprod)
+        self.lambda_t = torch.log(self.alpha_t) - torch.log(self.sigma_t)
+        self.model_outputs = [None] * solver_order
+        self.lower_order_nums = 0
+        self._orders: list = []
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        """:185-206: linspace(0, T-1, n+1) rounded, reversed, last dropped (no steps_offset); resets the history."""
+        self.num_inference_steps = num_inference_steps
+        T = self.config["num_train_timesteps"]
+        ts = np.linspace(0, T - 1, num_inference_steps + 1).round()[::-1][:-1].copy().astype(np.int64)
+        self.timesteps = torch.from_numpy(ts)
+        self.model_outputs = [None] * self.config["solver_order"]
+        self.lower_order_nums = 0
+        n = len(ts)
+        self._orders = [self._order_at(i, n, min(i, self.config["solver_order"])) for i in range(n)]
+        self._finish_set_timesteps(device)
+
+    def _needs_noise(self, t: int) -> bool:
+        return False   # an ODE solver: nothing is drawn after the initial latents
+
+    def _order_at(self, i: int, n: int, lower_order_nums: int) -> int:
+        """The update order :476-487 picks at step index i of n with `lower_order_nums` earlier steps counted."""
+        cfg = self.config
+        low = cfg["lower_order_final"] and n < 15
+        if cfg["solver_order"] == 1 or lower_order_nums < 1 or (low and i == n - 1):
+            return 1
+        if cfg["solver_order"] == 2 or lower_order_nums < 2 or (low and i == n - 2):
+            return 2
+        return 3
+
+    def order_at(self, i: int) -> int:
+        """Order of step i in a loop started by `set_timesteps`."""
+        return self._orders[i]
+
+    def _table_rows(self) -> list:
+        return [self._coefficients_at(i, self._orders[i]) for i in range(len(self._t_list))]
+
+    def _coefficients_at(self, i: int, order: int, timestep: Optional[int] = None) -> torch.Tensor:
+        """The fp32 scalars of step index i at `order` (:243-281, :305-427, same torch ops in the same order).
+        `timestep` overrides timesteps[i] for a step at a timestep outside the grid (the reference then takes the
+        last index)."""
+        cfg = self.config
+        tl = self._t_list
+        s0 = tl[i] if timestep is None else int(timestep)
+        t = 0 if i == len(tl) - 1 else tl[i + 1]   # :463
+        one, zero = torch.tensor(1.0), torch.tensor(0.0)
+        pp = cfg["algorithm_type"] == "dpmsolver++"
+        pred = cfg["prediction_type"]
+        a_s0, sg_s0 = self.alpha_t[s0], self.sigma_t[s0]
+        if pp:
+            c_a, c_b, c_d = {"epsilon": (one, -sg_s0, a_s0), "sample": (zero, one, one),
+                             "v_prediction": (a_s0, -sg_s0, one)}[pred]
+        else:
+            c_a, c_b, c_d = {"epsilon": (zero, one, one), "sample": (one, -a_s0, sg_s0),
+                             "v_prediction": (sg_s0, a_s0, one)}[pred]
+        lambda_t, lambda_s0 = self.lambda_t[t], self.lambda_t[s0]
+        alpha_t, alpha_s0 = self.alpha_t[t], self.alpha_t[s0]
+        sigma_t, sigma_s0 = self.sigma_t[t], self.sigma_t[s0]
+        h = lambda_t - lambda_s0
+        if pp:
+            c_s, c_0 = sigma_t / sigma_s0, alpha_t * (torch.exp(-h) - 1.0)
+        else:
+            c_s, c_0 = alpha_t / alpha_s0, sigma_t * (torch.exp(h) - 1.0)
+        c_1 = c_2 = inv_r0 = inv_r1 = w_r = inv_r01 = zero
+        if order == 2:
+            lambda_s1 = self.lambda_t[tl[i - 1]]
+            h_0 = lambda_s0 - lambda_s1
+            r0 = h_0 / h
+            inv_r0 = 1.0 / r0
+            if pp and cfg["solver_type"] == "midpoint":
+                c_1 = -(0.5 * (alpha_t * (torch.exp(-h) - 1.0)))
+            elif pp:
+                c_1 = alpha_t * ((torch.exp(-h) - 1.0) / h + 1.0)
+            elif cfg["solver_type"] == "midpoint":
+                c_1 = -(0.5 * (sigma_t * (torch.exp(h) - 1.0)))
+            else:
+                c_1 = -(sigma_t * ((torch.exp(h) - 1.0) / h - 1.0))
+        elif order == 3:
+            lambda_s1, lambda_s2 = self.lambda_t[tl[i - 1]], self.lambda_t[tl[i - 2]]
+            h_0, h_1 = lambda_s0 - lambda_s1, lambda_s1 - lambda_s2
+            r0, r1 = h_0 / h, h_1 / h
+            inv_r0, inv_r1 = 1.0 / r0, 1.0 / r1
+            w_r, inv_r01 = r0 / (r0 + r1), 1.0 / (r0 + r1)
+            if pp:
+                c_1 = alpha_t * ((torch.exp(-h) - 1.0) / h + 1.0)
+                c_2 = alpha_t * ((torch.exp(-h) - 1.0 + h) / h ** 2 - 0.5)
+            else:
+                c_1 = -(sigma_t * ((torch.exp(h) - 1.0) / h - 1.0))
+                c_2 = sigma_t * ((torch.exp(h) - 1.0 - h) / h ** 2 - 0.5)
+        return torch.stack([c_a, c_b, c_d, c_s, c_0, c_1, c_2, inv_r0, inv_r1, w_r, inv_r01]).float()
+
+    def _history(self, bufs, sample) -> list:
+        """The loop's `solver_order` persistent NCHW fp32 history slots, kept with the other buffers of this shape."""
+        hist = bufs.__dict__.setdefault("dpm_history", [])
+        while len(hist) < self.config["solver_order"]:
+            hist.append(torch.zeros(sample.shape, device=sample.device, dtype=torch.float32))
+        return hist
+
+    def _loop_step(self, i: int, model_out, cfg: bool, guidance: float, sample, noise, coef, next_in, bufs, *, B, Cc,
+                   HW, split_off):
+        """Step i of AudioDiffusion.inference: the converted output goes to slot i mod k of k = solver_order
+        history slots, the previous ones are read from slots i-1 and i-2 mod k."""
+        hist = self._history(bufs, sample)
+        k, order = self.config["solver_order"], self._orders[i]
+        m1 = hist[(i - 1) % k] if order >= 2 else None
+        m2 = hist[(i - 2) % k] if order >= 3 else None
+        L.dpm_step(model_out, cfg, guidance, sample, coef[i], order, hist[i % k], m1, m2, sample, next_in, B=B, Cc=Cc,
+                   HW=HW, split_off=split_off)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True, **_unused):
+        """:429-495 for NCHW fp32 CUDA tensors: converts the model output, shifts it into `model_outputs`, takes the
+        update of the order `lower_order_nums` and the final-step rules select, and counts `lower_order_nums`."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the"
+                             " scheduler")
+        L.require_cuda(model_output)   # no CPU fallback
+        t = int(timestep)
+        n = len(self._t_list)
+        i = self._t_index.get(t, n - 1)
+        k = self.config["solver_order"]
+        order = self._order_at(i, n, self.lower_order_nums)
+        if t == self._t_list[i] and order == self._orders[i]:
+            coef = self.coefficient_table(sample.device)[i]
+        else:
+            coef = self._coefficients_at(i, order, t).to(sample.device)
+        B, Cc, H, W = sample.shape
+        m0 = torch.empty(sample.shape, device=sample.device, dtype=torch.float32)
+        self.model_outputs = self.model_outputs[1:] + [m0]
+        m1 = self.model_outputs[-2] if order >= 2 else None
+        m2 = self.model_outputs[-3] if order >= 3 else None
+        mo = model_output.float().permute(0, 2, 3, 1).contiguous().view(B * H * W, Cc)   # channels-last rows
+        prev = torch.empty_like(sample, dtype=torch.float32)
+        L.dpm_step(mo, False, 1.0, sample.contiguous().float(), coef, order, m0, m1, m2, prev, None, B=B, Cc=Cc,
+                   HW=H * W)
+        if self.lower_order_nums < k:
+            self.lower_order_nums += 1
+        if not return_dict:
+            return (prev,)
+        return SchedulerOutput(prev_sample=prev)
