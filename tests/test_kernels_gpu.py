@@ -246,7 +246,9 @@ def attn_ref(q, k, v, heads, scale, bias=None):
 
 
 @pytest.mark.parametrize("B,heads,Lq,Lk,masked", [(2, 2, 300, 300, False), (1, 5, 4096, 4096, False),
-                                                   (2, 4, 200, 64, True), (3, 1, 8, 8, False), (2, 2, 130, 77, True)])
+                                                   (2, 4, 200, 64, True), (3, 1, 8, 8, False), (2, 2, 130, 77, True),
+                                                   (2, 2, 127, 65, False), (3, 2, 1, 7, False), (1, 20, 129, 77, True),
+                                                   (2, 1, 129, 1, False)])
 def test_attention(cuda, B, heads, Lq, Lk, masked):
     Cc = heads * 64
     g = torch.Generator(device="cpu").manual_seed(Lq + Lk)
