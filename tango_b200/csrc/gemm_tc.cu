@@ -14,7 +14,6 @@
 // See include/tango_b200.h (tng_conv_gemm) for the operator contract and the reference call sites it replaces.
 #include "tng_ptx.cuh"
 #include "tng_internal.h"
-#include <stdlib.h>
 
 namespace tng {
 
@@ -55,8 +54,7 @@ struct GemmKernelParams {
   int act;
   float act_param;
   int split_off;
-  int vec_ok;    // all row strides / bases allow 16-byte vector access
-  int fast_epi;  // vec_ok && Ncols % 4 == 0
+  int fast_epi;  // Ncols % 4 == 0 and every epilogue row stride and base allows 16-byte vector access
   // GroupNorm statistics of the fp32 output, emitted from the epilogue (full-tile launches only, see the host side):
   // col_stats[(img * Ncols + col) * 2 + {0, 1}] += sum / sum of squares over the rows of image img = row / stats_hw
   double* col_stats;
@@ -73,231 +71,52 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 /*barriers*/;
 };
 
-struct EpiRows {
-  long long row[ES];
-  int img[ES];
-  uint32_t valid;
-};
+// Chunk shapes of the epilogue (epi_tile). FULL: every row slot and column of the chunk is valid and 16-byte aligned,
+// fixed at compile time, so the code carries no predicates. VEC: 16-byte accesses, rows and columns predicated (partial
+// tiles, split-K). SCALAR: one access per element (Ncols % 4 != 0 or misaligned operands).
+enum EpiShape { EPI_SCALAR, EPI_VEC, EPI_FULL };
 
-// One 16-row x 32-column chunk, already staged (swizzled) in `st`: lanes (rsub = lane >> 3, cg = lane & 7) own the
-// 4 columns [4cg, 4cg+4) of rows 4i + rsub, i = 0..3.
-template <bool RES, bool F32, bool BF16, bool VEC>
-__device__ __forceinline__ void epi_chunk(const GemmKernelParams& p, const float* st, const EpiRows& R, int rsub, int cg,
-                                          int col) {
-  const bool col_ok = col < p.Ncols;
-  const bool has_res = RES && (p.res != nullptr);
-  const bool has_acc = F32 && (p.accumulate != 0);
-  const bool has_f32 = F32 && (p.out_f32 != nullptr);
-  const bool has_bf = BF16 && (p.out_bf16 != nullptr);
-  // ---- all global loads of the chunk first (independent -> in flight together)
-  float4 rres[ES], rold[ES];
-  if (has_res) {
+__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+__device__ __forceinline__ float4 scale4(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
+
+// act_f over a chunk, with the activation fixed at compile time
+template <int ACT>
+__device__ __forceinline__ void act_chunk(float4 (&a)[ES], float ap) {
 #pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (col_ok && ((R.valid >> i) & 1)) {
-        if (VEC) {
-          if (p.res_bf16) r4 = load_bf16x4(reinterpret_cast<const __nv_bfloat16*>(p.res) + R.row[i] * p.ldr + col);
-          else r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + R.row[i] * p.ldr + col);
-        } else {
-          float t[4] = {0.f, 0.f, 0.f, 0.f};
-          for (int j = 0; j < 4; ++j)
-            if (col + j < p.Ncols)
-              t[j] = p.res_bf16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.res)[R.row[i] * p.ldr + col + j])
-                                : reinterpret_cast<const float*>(p.res)[R.row[i] * p.ldr + col + j];
-          r4 = make_float4(t[0], t[1], t[2], t[3]);
-        }
-      }
-      rres[i] = r4;
-    }
-  }
-  if (has_acc) {
-#pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (col_ok && ((R.valid >> i) & 1)) {
-        if (VEC) {
-          r4 = *reinterpret_cast<const float4*>(p.out_f32 + R.row[i] * p.ld_f32 + col);
-        } else {
-          float t[4] = {0.f, 0.f, 0.f, 0.f};
-          for (int j = 0; j < 4; ++j)
-            if (col + j < p.Ncols) t[j] = p.out_f32[R.row[i] * p.ld_f32 + col + j];
-          r4 = make_float4(t[0], t[1], t[2], t[3]);
-        }
-      }
-      rold[i] = r4;
-    }
-  }
-  float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (p.bias && col_ok) {
-    if (VEC) {
-      b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-    } else {
-      float t[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int j = 0; j < 4; ++j)
-        if (col + j < p.Ncols) t[j] = __ldg(p.bias + col + j);
-      b4 = make_float4(t[0], t[1], t[2], t[3]);
-    }
-  }
-  const bool has_rv = (p.rowvec != nullptr);
-  const float alpha = p.alpha;
-#pragma unroll
-  for (int i = 0; i < ES; ++i) {
-    const int r = 4 * i + rsub;
-    float4 a = *reinterpret_cast<const float4*>(st + r * 32 + ((cg ^ (r & 7)) << 2));
-    if (!col_ok || !((R.valid >> i) & 1)) continue;
-    a.x += b4.x; a.y += b4.y; a.z += b4.z; a.w += b4.w;
-    if (has_rv) {
-      const float* rv = p.rowvec + static_cast<long long>(R.img[i]) * p.rowvec_ld + col;
-      if (VEC) {
-        const float4 r4 = __ldg(reinterpret_cast<const float4*>(rv));
-        a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
-      } else {
-        if (col + 0 < p.Ncols) a.x += __ldg(rv + 0);
-        if (col + 1 < p.Ncols) a.y += __ldg(rv + 1);
-        if (col + 2 < p.Ncols) a.z += __ldg(rv + 2);
-        if (col + 3 < p.Ncols) a.w += __ldg(rv + 3);
-      }
-    }
-    if (has_res) { a.x += rres[i].x; a.y += rres[i].y; a.z += rres[i].z; a.w += rres[i].w; }
-    a.x *= alpha; a.y *= alpha; a.z *= alpha; a.w *= alpha;
-    if (has_f32) {
-      if (has_acc) { a.x += rold[i].x; a.y += rold[i].y; a.z += rold[i].z; a.w += rold[i].w; }
-      float* op = p.out_f32 + R.row[i] * p.ld_f32 + col;
-      if (VEC) {
-        *reinterpret_cast<float4*>(op) = a;
-      } else {
-        const float t[4] = {a.x, a.y, a.z, a.w};
-        for (int j = 0; j < 4; ++j)
-          if (col + j < p.Ncols) op[j] = t[j];
-      }
-    }
-    if (has_bf) {
-      __nv_bfloat16* op = p.out_bf16 + R.row[i] * p.ld_bf16 + col;
-      const float y0 = act_f(a.x, p.act, p.act_param), y1 = act_f(a.y, p.act, p.act_param);
-      const float y2 = act_f(a.z, p.act, p.act_param), y3 = act_f(a.w, p.act, p.act_param);
-      if (VEC) {
-        store4_split(op, make_float4(y0, y1, y2, y3), p.split_off);
-      } else {
-        const float t[4] = {y0, y1, y2, y3};
-        for (int j = 0; j < 4; ++j)
-          if (col + j < p.Ncols) store_bf16_split(op + j, t[j], p.split_off);
-      }
-    }
-  }
+  for (int i = 0; i < ES; ++i)
+    a[i] = make_float4(act_f(a[i].x, ACT, ap), act_f(a[i].y, ACT, ap), act_f(a[i].z, ACT, ap), act_f(a[i].w, ACT, ap));
 }
 
-// Lean path for FULL tiles (all 128 rows valid, all 32 columns of the chunk < Ncols, 16-byte aligned): the rows of a
-// tile are consecutive output rows (the host tiling guarantees it), so slot i of a lane is row r0 + 4i and every
-// pointer advances by a constant stride — a few instructions per 16-byte access, no per-element predicates.
-template <bool RES, bool F32, bool BF16>
-__device__ __forceinline__ void epi_chunk_full(const GemmKernelParams& p, const float* st, long long r0, int img0,
-                                               int rsub, int cg, int col, bool rv_uniform, long long stats_img) {
-  float4 add4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (p.bias) add4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-  if (p.rowvec && rv_uniform) {
-    const float4 r4 = __ldg(reinterpret_cast<const float4*>(p.rowvec + static_cast<long long>(img0) * p.rowvec_ld + col));
-    add4.x += r4.x; add4.y += r4.y; add4.z += r4.z; add4.w += r4.w;
-  }
-  float4 rres[ES];
-  if (RES) {
-    if (p.res_bf16) {
-      const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + r0 * p.ldr + col;
-      const long long rs = 4 * p.ldr;
+// Row r, columns [4cg, 4cg + 4) of a warp's 16 x 32 staging tile (layout: epi_stage)
+__device__ __forceinline__ float4 staged(const float* st, int r, int cg) {
+  return *reinterpret_cast<const float4*>(st + r * 32 + ((cg ^ (r & 7)) << 2));
+}
+
+// The first n (<= 4) values at q (fp32 or bf16) as fp32, zero-filled; one vector load when VEC (n is 4 there). RO
+// reads through the read-only cache: bias and rowvec only, never the residual or the old output, which the kernel may
+// be writing.
+template <bool VEC, bool RO = false, typename T>
+__device__ __forceinline__ float4 load4(const T* q, int n) {
+  if constexpr (VEC && sizeof(T) == 2) return load_bf16x4(q);
+  if constexpr (VEC && sizeof(T) == 4)
+    return RO ? __ldg(reinterpret_cast<const float4*>(q)) : *reinterpret_cast<const float4*>(q);
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-      for (int i = 0; i < ES; ++i) rres[i] = load_bf16x4(rp + i * rs);
-    } else {
-      const float* rp = reinterpret_cast<const float*>(p.res) + r0 * p.ldr + col;
-      const long long rs = 4 * p.ldr;
-#pragma unroll
-      for (int i = 0; i < ES; ++i) rres[i] = *reinterpret_cast<const float4*>(rp + i * rs);
-    }
-  }
-  float4 a[ES];
-#pragma unroll
-  for (int i = 0; i < ES; ++i) {
-    const int r = 4 * i + rsub;
-    a[i] = *reinterpret_cast<const float4*>(st + r * 32 + ((cg ^ (r & 7)) << 2));
-    a[i].x += add4.x; a[i].y += add4.y; a[i].z += add4.z; a[i].w += add4.w;
-  }
-  if (p.rowvec && !rv_uniform) {
-#pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      const int im = img0 + (4 * i) / (p.bw * p.bh);  // img0 is the image of slot 0; rows advance by 4 per slot
-      const float4 r4 = __ldg(reinterpret_cast<const float4*>(p.rowvec + static_cast<long long>(im) * p.rowvec_ld + col));
-      a[i].x += r4.x; a[i].y += r4.y; a[i].z += r4.z; a[i].w += r4.w;
-    }
-  }
-  if (RES) {
-#pragma unroll
-    for (int i = 0; i < ES; ++i) { a[i].x += rres[i].x; a[i].y += rres[i].y; a[i].z += rres[i].z; a[i].w += rres[i].w; }
-  }
-  if (p.alpha != 1.0f) {
-    const float al = p.alpha;
-#pragma unroll
-    for (int i = 0; i < ES; ++i) { a[i].x *= al; a[i].y *= al; a[i].z *= al; a[i].w *= al; }
-  }
-  if (F32) {
-    float* op = p.out_f32 + r0 * p.ld_f32 + col;
-    const long long os = 4 * p.ld_f32;
-    if (p.accumulate) {
-#pragma unroll
-      for (int i = 0; i < ES; ++i) {
-        const float4 o4 = *reinterpret_cast<const float4*>(op + i * os);
-        a[i].x += o4.x; a[i].y += o4.y; a[i].z += o4.z; a[i].w += o4.w;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < ES; ++i) *reinterpret_cast<float4*>(op + i * os) = a[i];
-  }
-  if (p.col_stats) {
-    // Column sums of this warp's 16 rows x 32 columns (all rows belong to image stats_img): 4 rows in registers,
-    // then across the four row-lanes (lane bits 3 and 4); lanes 0..7 hold the totals of their 4 columns and add
-    // them to the fp64 per-(image, channel) accumulators — fp32 partials over 16 values, fp64 across tiles.
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
-#pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      s0 += a[i].x; s1 += a[i].y; s2 += a[i].z; s3 += a[i].w;
-      q0 = fmaf(a[i].x, a[i].x, q0); q1 = fmaf(a[i].y, a[i].y, q1);
-      q2 = fmaf(a[i].z, a[i].z, q2); q3 = fmaf(a[i].w, a[i].w, q3);
-    }
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o); s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-      s2 += __shfl_xor_sync(0xffffffffu, s2, o); s3 += __shfl_xor_sync(0xffffffffu, s3, o);
-      q0 += __shfl_xor_sync(0xffffffffu, q0, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-      q2 += __shfl_xor_sync(0xffffffffu, q2, o); q3 += __shfl_xor_sync(0xffffffffu, q3, o);
-    }
-    if (rsub == 0) {
-      double* sp = p.col_stats + (stats_img * p.Ncols + col) * 2;
-      atomicAdd(sp + 0, static_cast<double>(s0)); atomicAdd(sp + 1, static_cast<double>(q0));
-      atomicAdd(sp + 2, static_cast<double>(s1)); atomicAdd(sp + 3, static_cast<double>(q1));
-      atomicAdd(sp + 4, static_cast<double>(s2)); atomicAdd(sp + 5, static_cast<double>(q2));
-      atomicAdd(sp + 6, static_cast<double>(s3)); atomicAdd(sp + 7, static_cast<double>(q3));
-    }
-  }
-  if (BF16) {
-    if (p.act == TNG_ACT_SILU) {
-#pragma unroll
-      for (int i = 0; i < ES; ++i) { a[i].x = silu_f(a[i].x); a[i].y = silu_f(a[i].y); a[i].z = silu_f(a[i].z); a[i].w = silu_f(a[i].w); }
-    } else if (p.act == TNG_ACT_LRELU) {
-      const float sl = p.act_param;
-#pragma unroll
-      for (int i = 0; i < ES; ++i) {
-        a[i].x = a[i].x > 0.f ? a[i].x : a[i].x * sl; a[i].y = a[i].y > 0.f ? a[i].y : a[i].y * sl;
-        a[i].z = a[i].z > 0.f ? a[i].z : a[i].z * sl; a[i].w = a[i].w > 0.f ? a[i].w : a[i].w * sl;
-      }
-    }
-    __nv_bfloat16* op = p.out_bf16 + r0 * p.ld_bf16 + col;
-    const long long os = 4 * p.ld_bf16;
-#pragma unroll
-    for (int i = 0; i < ES; ++i) store4_bf16(op + i * os, a[i]);
-    if (p.split_off > 0) {
-      op += p.split_off;
-#pragma unroll
-      for (int i = 0; i < ES; ++i) store4_bf16_lo(op + i * os, a[i]);
-    }
-  }
+  for (int j = 0; j < 4; ++j)
+    if (j < n) t[j] = static_cast<float>(RO ? __ldg(q + j) : q[j]);
+  return make_float4(t[0], t[1], t[2], t[3]);
+}
+
+template <bool VEC>
+__device__ __forceinline__ float4 load_bias(const GemmKernelParams& p, int col, int n) {
+  return p.bias ? load4<VEC, true>(p.bias + col, n) : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// the residual at element offset off
+template <bool VEC>
+__device__ __forceinline__ float4 load_res(const GemmKernelParams& p, long long off, int n) {
+  return p.res_bf16 ? load4<VEC>(static_cast<const __nv_bfloat16*>(p.res) + off, n)
+                    : load4<VEC>(static_cast<const float*>(p.res) + off, n);
 }
 
 // 32 accumulator columns of this warp (8-column groups 4c .. 4c+3 = registers v[0, 16), see tng_ptx.cuh) -> the warp's
@@ -324,104 +143,169 @@ __device__ __forceinline__ void stage_chunk(float* st, int lane, const float (&a
   __syncwarp();
 }
 
-template <int BN, bool RES, bool F32, bool BF16>
-__device__ __forceinline__ void epi_tile_full(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2], long long r0,
-                                              int img0, bool rv_uniform, int tn, int lane, long long stats_img) {
-  const int cg = lane & 7, rsub = lane >> 3;
-#pragma unroll 1
-  for (int c = 0; c < BN / 32; ++c) {
-    stage_chunk<BN>(st, lane, acc, c);
-    epi_chunk_full<RES, F32, BF16>(p, st, r0, img0, rsub, cg, tn * BN + 32 * c + 4 * cg, rv_uniform, stats_img);
-  }
-}
+// The current work item as the epilogue sees it: the tile's rows are the consecutive output rows starting at row_base,
+// of which the first nvalid are valid (see the host tiling); tile row r lies in image n0 + r / (bw * bh). tn = N tile,
+// sp = K half under split-K.
+struct EpiTile {
+  long long row_base;
+  int n0, nvalid, tn, sp;
+};
 
-template <int BN, bool VEC>
-__device__ __forceinline__ void epi_tile_generic(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2],
-                                                 const EpiRows& R, int tn, int lane) {
+// Epilogue of one non-GEGLU tile, 32 columns per chunk. MODE bits: 1 residual, 2 fp32 output, 4 bf16 output. FULL tiles
+// compile in exactly the parts the launch uses; the other shapes compile in all three and test the pointers.
+// Lane (rsub = lane >> 3, cg = lane & 7) owns columns [col, col + 4) of tile rows wr + rsub + 4i, i < ES:
+//   out = ((((acc + bias) + rowvec[image]) + res) * alpha) [+ out when accumulating]
+// Split-K: each K half red.adds alpha * its partial into an fp32 output the host zeroed, and only half 0 adds the bias,
+// rowvec and residual. With exactly two partials per element the result does not depend on their order (0 + a + b,
+// fp32 addition commutes), so runs stay reproducible.
+// All global loads of a chunk are issued before its first store: res may be out_f32 (the transformer out-projections).
+template <int BN, int SHAPE, int MODE>
+__device__ __forceinline__ void epi_tile(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2], const EpiTile& t,
+                                         int wr, int lane) {
+  constexpr bool FULL = SHAPE == EPI_FULL, VEC = SHAPE != EPI_SCALAR;
   const int cg = lane & 7, rsub = lane >> 3;
+  const int trow = wr + rsub;                 // tile row of slot 0
+  const long long r0 = t.row_base + trow;     // output row of slot 0
+  const int lane_rows = FULL ? ES : min(ES, max(0, (t.nvalid - trow + 3) >> 2));   // valid slots: a prefix
+  const bool red = SHAPE == EPI_VEC && p.ksplit > 1;   // split-K tiles: never FULL, always 16-byte aligned (host)
+  const bool add_terms = !red || t.sp == 0;
+  const bool has_res = (MODE & 1) && (FULL || p.res) && add_terms;
+  const bool has_f32 = (MODE & 2) && (FULL || p.out_f32);
+  const bool has_bf = (MODE & 4) && (FULL || p.out_bf16);
+  const bool has_rv = p.rowvec && add_terms;
+  const int rpi = p.bw * p.bh;   // rows of one image inside a tile: a power of two (host tiling)
+  const int rpi_log2 = __ffs(rpi) - 1;
+  // image of the warp's 16 rows for the GroupNorm statistics (stats_hw % 16 == 0: host check)
+  const long long simg = (FULL && p.col_stats) ? (t.row_base + wr) / p.stats_hw : 0;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 1
   for (int c = 0; c < BN / 32; ++c) {
     stage_chunk<BN>(st, lane, acc, c);
-    epi_chunk<true, true, true, VEC>(p, st, R, rsub, cg, tn * BN + 32 * c + 4 * cg);
-  }
-}
-
-// Split-K epilogue: this CTA holds the partial sum over its half of K. out (+)= alpha * (partial [+ bias + rowvec + res
-// for the first half only]) with fp32 red.adds into an output the host zeroed beforehand. With exactly two partials
-// per element the result does not depend on their order (0 + a + b, fp32 addition commutes), so runs stay
-// reproducible. Used for under-filled launches with a long reduction (the 32x2 level of the UNet): the epilogue is
-// small next to the main loop, so this is the simple row-slot form. wr = first tile row of this warp.
-template <int BN>
-__device__ __forceinline__ void epi_tile_splitk(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2],
-                                                long long row_base, int n0, int rpi, int nvalid, int sp, int tn, int lane,
-                                                int wr) {
-  const int cg = lane & 7, rsub = lane >> 3;
-#pragma unroll 1
-  for (int c = 0; c < BN / 32; ++c) {
-    stage_chunk<BN>(st, lane, acc, c);
-    const int col = tn * BN + 32 * c + 4 * cg;
-    const bool col_ok = col < p.Ncols;   // Ncols % 4 == 0 (checked on the host)
-    float4 add4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (col_ok && sp == 0 && p.bias) add4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-#pragma unroll 1
-    for (int i = 0; i < ES; ++i) {
-      const int rr = wr + 4 * i + rsub;
-      if (!col_ok || rr >= nvalid) continue;
-      const long long row = row_base + rr;
-      float4 a = *reinterpret_cast<const float4*>(st + (4 * i + rsub) * 32 + ((cg ^ ((4 * i + rsub) & 7)) << 2));
-      if (sp == 0) {
-        a.x += add4.x; a.y += add4.y; a.z += add4.z; a.w += add4.w;
-        if (p.rowvec) {
-          const float4 r4 = __ldg(reinterpret_cast<const float4*>(p.rowvec + static_cast<long long>(n0 + rr / rpi) * p.rowvec_ld + col));
-          a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
-        }
-        if (p.res) {
-          if (p.res_bf16) {
-            const float4 r4 = load_bf16x4(reinterpret_cast<const __nv_bfloat16*>(p.res) + row * p.ldr + col);
-            a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
-          } else {
-            const float4 r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + row * p.ldr + col);
-            a.x += r4.x; a.y += r4.y; a.z += r4.z; a.w += r4.w;
-          }
+    const int col = t.tn * BN + 32 * c + 4 * cg;
+    const int ncols = FULL ? 4 : min(4, p.Ncols - col);   // valid columns of the lane, none when <= 0
+    const int nrows = ncols > 0 ? lane_rows : 0;
+    float4 res[ES];
+    if (has_res) {
+      const long long off = r0 * p.ldr + col, rs = 4 * p.ldr;
+#pragma unroll
+      for (int i = 0; i < ES; ++i) res[i] = i < nrows ? load_res<VEC>(p, off + i * rs, ncols) : zero;
+    }
+    const float4 b4 = (add_terms && ncols > 0) ? load_bias<VEC>(p, col, ncols) : zero;
+    // branch-free, so that the four staging reads issue together (one branch between them costs ~5 % on the
+    // HBM-bound GEMMs)
+    float4 a[ES];
+#pragma unroll
+    for (int i = 0; i < ES; ++i) a[i] = add4(staged(st, 4 * i + rsub, cg), b4);
+    if (has_rv) {
+      float4 rv = zero;
+#pragma unroll
+      for (int i = 0; i < ES; ++i) {
+        if (i >= nrows) continue;
+        // image n0 + (tile row) / rpi; when rpi % 16 == 0 the warp's 16 rows lie in one image, loaded by slot 0
+        const long long img = t.n0 + ((trow + 4 * i) >> rpi_log2);
+        if (i == 0 || rpi % 16 != 0) rv = load4<VEC, true>(p.rowvec + img * p.rowvec_ld + col, ncols);
+        a[i] = add4(a[i], rv);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < ES; ++i) a[i] = scale4(has_res ? add4(a[i], res[i]) : a[i], p.alpha);
+    if (has_f32) {
+      float* op = p.out_f32 + r0 * p.ld_f32 + col;
+      const long long os = 4 * p.ld_f32;
+      if (p.accumulate) {
+#pragma unroll
+        for (int i = 0; i < ES; ++i)
+          if (i < nrows) a[i] = add4(a[i], load4<VEC>(op + i * os, ncols));
+      }
+#pragma unroll
+      for (int i = 0; i < ES; ++i) {
+        if (i >= nrows) continue;
+        float* q = op + i * os;
+        if (red) {
+          atomicAdd(q, a[i].x); atomicAdd(q + 1, a[i].y); atomicAdd(q + 2, a[i].z); atomicAdd(q + 3, a[i].w);
+        } else if (VEC) {
+          *reinterpret_cast<float4*>(q) = a[i];
+        } else {
+          const float v[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (j < ncols) q[j] = v[j];
         }
       }
-      a.x *= p.alpha; a.y *= p.alpha; a.z *= p.alpha; a.w *= p.alpha;
-      float* op = p.out_f32 + row * p.ld_f32 + col;
-      atomicAdd(op, a.x); atomicAdd(op + 1, a.y); atomicAdd(op + 2, a.z); atomicAdd(op + 3, a.w);
+    }
+    if (FULL && p.col_stats) {
+      // Column sums of this warp's 16 rows x 32 columns (all rows belong to image simg): 4 rows in registers,
+      // then across the four row-lanes (lane bits 3 and 4); lanes 0..7 hold the totals of their 4 columns and add
+      // them to the fp64 per-(image, channel) accumulators — fp32 partials over 16 values, fp64 across tiles.
+      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
+#pragma unroll
+      for (int i = 0; i < ES; ++i) {
+        s0 += a[i].x; s1 += a[i].y; s2 += a[i].z; s3 += a[i].w;
+        q0 = fmaf(a[i].x, a[i].x, q0); q1 = fmaf(a[i].y, a[i].y, q1);
+        q2 = fmaf(a[i].z, a[i].z, q2); q3 = fmaf(a[i].w, a[i].w, q3);
+      }
+#pragma unroll
+      for (int o = 8; o <= 16; o <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o); s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o); s3 += __shfl_xor_sync(0xffffffffu, s3, o);
+        q0 += __shfl_xor_sync(0xffffffffu, q0, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+        q2 += __shfl_xor_sync(0xffffffffu, q2, o); q3 += __shfl_xor_sync(0xffffffffu, q3, o);
+      }
+      if (rsub == 0) {
+        double* sp = p.col_stats + (simg * p.Ncols + col) * 2;
+        atomicAdd(sp + 0, static_cast<double>(s0)); atomicAdd(sp + 1, static_cast<double>(q0));
+        atomicAdd(sp + 2, static_cast<double>(s1)); atomicAdd(sp + 3, static_cast<double>(q1));
+        atomicAdd(sp + 4, static_cast<double>(s2)); atomicAdd(sp + 5, static_cast<double>(q2));
+        atomicAdd(sp + 6, static_cast<double>(s3)); atomicAdd(sp + 7, static_cast<double>(q3));
+      }
+    }
+    if (has_bf) {
+      // one branch on p.act per chunk: a branch per element makes the bf16-output GEMMs ~30 % slower
+      if (p.act == TNG_ACT_SILU) act_chunk<TNG_ACT_SILU>(a, p.act_param);
+      else if (p.act == TNG_ACT_LRELU) act_chunk<TNG_ACT_LRELU>(a, p.act_param);
+      __nv_bfloat16* op = p.out_bf16 + r0 * p.ld_bf16 + col;
+      const long long os = 4 * p.ld_bf16;
+#pragma unroll
+      for (int i = 0; i < ES; ++i) {
+        if (i >= nrows) continue;
+        if (VEC) {
+          store4_bf16(op + i * os, a[i]);
+        } else {
+          const float v[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (j < ncols) store_bf16_split(op + i * os + j, v[j], p.split_off);
+        }
+      }
+      if (VEC && p.split_off > 0) {
+#pragma unroll
+        for (int i = 0; i < ES; ++i)
+          if (i < nrows) store4_bf16_lo(op + p.split_off + i * os, a[i]);
+      }
     }
   }
 }
 
 // GEGLU: columns [0, BN/2) of the tile are "hidden", [BN/2, BN) the matching "gate" (weights interleaved on the
-// host). out[:, tn*BN/2 + j] = (hid + b) * gelu_erf(gate + b'). Rows r0 + 4i (consecutive-row tiles); rows >= nvalid
-// are skipped.
+// host). out[:, tn*BN/2 + j] = (hid + b) * gelu_erf(gate + b'). Rows past nvalid are skipped unless FULL.
 template <int BN, bool FULL, bool SPLIT, bool TANH>
-__device__ __forceinline__ void epi_tile_geglu(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2], long long r0,
-                                               int nleft, int tn, int lane) {
+__device__ __forceinline__ void epi_tile_geglu(const GemmKernelParams& p, float* st, const float (&acc)[BN / 2],
+                                               const EpiTile& t, int wr, int lane) {
   constexpr int HALF = BN / 2;
   const int cg = lane & 7, rsub = lane >> 3;
+  const int trow = wr + rsub;
 #pragma unroll 1
   for (int c = 0; c < HALF / 32; ++c) {
     float4 hid[ES], g[ES];
     stage_chunk<BN>(st, lane, acc, c);
 #pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      const int r = 4 * i + rsub;
-      hid[i] = *reinterpret_cast<const float4*>(st + r * 32 + ((cg ^ (r & 7)) << 2));
-    }
+    for (int i = 0; i < ES; ++i) hid[i] = staged(st, 4 * i + rsub, cg);
     stage_chunk<BN>(st, lane, acc, c + HALF / 32);
 #pragma unroll
-    for (int i = 0; i < ES; ++i) {
-      const int r = 4 * i + rsub;
-      g[i] = *reinterpret_cast<const float4*>(st + r * 32 + ((cg ^ (r & 7)) << 2));
-    }
-    const int gcol = tn * BN + 32 * c + 4 * cg;  // GEMM column of the hidden half; gate at + HALF
-    const int ocol = tn * HALF + 32 * c + 4 * cg;
-    float4 bh = make_float4(0.f, 0.f, 0.f, 0.f), bg = bh;
-    if (p.bias) {
-      bh = __ldg(reinterpret_cast<const float4*>(p.bias + gcol));
-      bg = __ldg(reinterpret_cast<const float4*>(p.bias + gcol + HALF));
-    }
+    for (int i = 0; i < ES; ++i) g[i] = staged(st, 4 * i + rsub, cg);
+    const int gcol = t.tn * BN + 32 * c + 4 * cg;  // GEMM column of the hidden half; gate at + HALF
+    const int ocol = t.tn * HALF + 32 * c + 4 * cg;
+    const float4 bh = load_bias<true>(p, gcol, 4), bg = load_bias<true>(p, gcol + HALF, 4);
     // branch-free arithmetic over all 16 values of this lane (independent MUFU chains to interleave)
 #pragma unroll
     for (int i = 0; i < ES; ++i) {
@@ -430,21 +314,26 @@ __device__ __forceinline__ void epi_tile_geglu(const GemmKernelParams& p, float*
       hid[i].z = (hid[i].z + bh.z) * (TANH ? gelu_tanh_f(g[i].z + bg.z) : gelu_erf_f(g[i].z + bg.z));
       hid[i].w = (hid[i].w + bh.w) * (TANH ? gelu_tanh_f(g[i].w + bg.w) : gelu_erf_f(g[i].w + bg.w));
     }
-    __nv_bfloat16* op = p.out_bf16 + r0 * p.ld_bf16 + ocol;
+    __nv_bfloat16* op = p.out_bf16 + (t.row_base + trow) * p.ld_bf16 + ocol;
     const long long os = 4 * p.ld_bf16;
 #pragma unroll
     for (int i = 0; i < ES; ++i) {
-      if (!FULL && 4 * i >= nleft) continue;
-      uint2 u;
-      u.x = pack_bf16(hid[i].x, hid[i].y); u.y = pack_bf16(hid[i].z, hid[i].w);
-      *reinterpret_cast<uint2*>(op + i * os) = u;
-      if (SPLIT) {
-        uint2 l;
-        l.x = pack_bf16_lo(hid[i].x, hid[i].y); l.y = pack_bf16_lo(hid[i].z, hid[i].w);
-        *reinterpret_cast<uint2*>(op + p.split_off + i * os) = l;
-      }
+      if (!FULL && trow + 4 * i >= t.nvalid) continue;
+      store4_bf16(op + i * os, hid[i]);
+      if (SPLIT) store4_bf16_lo(op + p.split_off + i * os, hid[i]);
     }
   }
+}
+
+// Work item `tile` (under split-K consecutive items are the K halves of one output tile): K half sp, N tile tn and the
+// origin (w0, h0, n0) of its M tile in the output pixel grid
+struct WorkItem {
+  int sp, tn, w0, h0, n0;
+};
+__device__ __forceinline__ WorkItem work_item(const GemmKernelParams& p, int tile) {
+  const int t2 = tile / p.ksplit, tm = t2 / p.n_tiles;
+  const int tw = tm % p.tiles_w, th = (tm / p.tiles_w) % p.tiles_h, tb = tm / (p.tiles_w * p.tiles_h);
+  return WorkItem{tile % p.ksplit, t2 % p.n_tiles, tw * p.bw, th * p.bh, tb * p.bn};
 }
 
 // K iterations of work item `tile` (all of them unless split-K)
@@ -495,14 +384,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
     if (tid == 0) {
       uint32_t n_loaded = 0;
       for (int tile = work0; tile < total_tiles; tile += work_stride) {
-        const int sp = tile % p.ksplit, t2 = tile / p.ksplit;
-        const int tm = t2 / p.n_tiles, tn = t2 % p.n_tiles;
-        const int tw = tm % p.tiles_w;
-        const int th = (tm / p.tiles_w) % p.tiles_h;
-        const int tb = tm / (p.tiles_w * p.tiles_h);
-        const int w0 = tw * p.bw, h0 = th * p.bh, n0 = tb * p.bn;
+        const WorkItem w = work_item(p, tile);
         const int nk = tile_kiters(p, tile);
-        int k = sp * p.total_kiters / p.ksplit, gi = 0;   // flat K iteration -> (k-group, K block)
+        int k = w.sp * p.total_kiters / p.ksplit, gi = 0;   // flat K iteration -> (k-group, K block)
         while (k >= p.g[gi].nkb) { k -= p.g[gi].nkb; ++gi; }
         for (int ki = 0; ki < nk; ++ki, ++k, ++n_loaded) {
           if (k == p.g[gi].nkb) { k = 0; ++gi; }
@@ -512,8 +396,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
           const KGroupDev g = p.g[gi];
           const CUtensorMap* am = g.view == 0 ? &amap0 : g.view == 1 ? &amap1 : g.view == 2 ? &amap2 : &amap3;
           mbar_arrive_expect_tx(&full_bar[slot], Cfg::STAGE_BYTES);
-          tma_load_4d(sA + slot * A_TILE_BYTES, am, &full_bar[slot], g.a_c0 + k * BK, w0 + g.dw, h0 + g.dh, n0);
-          tma_load_2d(sB + slot * Cfg::B_TILE_BYTES, &bmap, &full_bar[slot], g.b_k0 + k * BK, tn * BN);
+          tma_load_4d(sA + slot * A_TILE_BYTES, am, &full_bar[slot], g.a_c0 + k * BK, w.w0 + g.dw, w.h0 + g.dh, w.n0);
+          tma_load_2d(sB + slot * Cfg::B_TILE_BYTES, &bmap, &full_bar[slot], g.b_k0 + k * BK, w.tn * BN);
         }
       }
     }
@@ -524,7 +408,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
   // ===================================================== main loop + epilogue (consumer warpgroups 1 and 2)
   const int cw = warp - 4;                         // consumer warp 0..7
   float* st = sEpi + cw * (16 * 32);
-  const int rsub = lane >> 3;
   const int wr = 16 * cw;                          // first tile row of this warp
   const uint32_t a_off = static_cast<uint32_t>(wg - 1) * (64 * 128);   // rows [64 (wg-1), 64 wg) of the A tile
   const bool release = (tid & 127) == 0;           // the thread that arrives on the empty barriers for its warpgroup
@@ -535,8 +418,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   for (int tile = work0; tile < total_tiles; tile += work_stride) {
-    const int sp = tile % p.ksplit, t2 = tile / p.ksplit;
-    const int tm = t2 / p.n_tiles, tn = t2 % p.n_tiles;
     const int nk = tile_kiters(p, tile);
     for (int ki = 0; ki < nk; ++ki) {
       const int slot = static_cast<int>(n_used % STAGES);
@@ -561,57 +442,34 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
     mbar_arrive_if(&empty_bar[(n_used - 1) % STAGES], release);
 
     // ---- epilogue: rows of a tile are consecutive output rows; valid rows form a prefix (see host tiling)
-    const int tw = tm % p.tiles_w;
-    const int th = (tm / p.tiles_w) % p.tiles_h;
-    const int tb = tm / (p.tiles_w * p.tiles_h);
-    const int w0 = tw * p.bw, h0 = th * p.bh, n0 = tb * p.bn;
-    const long long row_base = (static_cast<long long>(n0) * p.H + h0) * p.W + w0;
+    const WorkItem w = work_item(p, tile);
     int nvalid;
-    if (p.bh == 1 && p.bn == 1) nvalid = min(BM, p.W - w0);
-    else if (p.bn == 1) nvalid = min(p.bh, p.H - h0) * p.bw;
-    else nvalid = min(p.bn, p.NB - n0) * p.bh * p.bw;
-    const int rpi = p.bw * p.bh;  // rows of one image inside a tile
-    const bool full = p.fast_epi && (nvalid == BM) && ((tn + 1) * BN <= p.Ncols);
-    if (p.ksplit > 1) {
-      epi_tile_splitk<BN>(p, st, acc, row_base, n0, rpi, nvalid, sp, tn, lane, wr);
-    } else if (geglu) {
-      // slot i of this lane is row wr + rsub + 4i; rows below nvalid are valid
+    if (p.bh == 1 && p.bn == 1) nvalid = min(BM, p.W - w.w0);
+    else if (p.bn == 1) nvalid = min(p.bh, p.H - w.h0) * p.bw;
+    else nvalid = min(p.bn, p.NB - w.n0) * p.bh * p.bw;
+    const EpiTile t{(static_cast<long long>(w.n0) * p.H + w.h0) * p.W + w.w0, w.n0, nvalid, w.tn, w.sp};
+    if (geglu) {
       if constexpr (BN == 128 || BN == 256) {   // the host only selects these N tiles for GEGLU
-        const long long gr0 = row_base + wr + rsub;
-        const int nleft = nvalid - (wr + rsub);
         if (p.act == TNG_ACT_GEGLU_TANH) {   // T5 front-end (small): one general instantiation
-          if (p.split_off > 0) epi_tile_geglu<BN, false, true, true>(p, st, acc, gr0, nleft, tn, lane);
-          else epi_tile_geglu<BN, false, false, true>(p, st, acc, gr0, nleft, tn, lane);
-        } else if (p.split_off > 0) epi_tile_geglu<BN, false, true, false>(p, st, acc, gr0, nleft, tn, lane);
-        else if (nvalid == BM) epi_tile_geglu<BN, true, false, false>(p, st, acc, gr0, nleft, tn, lane);
-        else epi_tile_geglu<BN, false, false, false>(p, st, acc, gr0, nleft, tn, lane);
+          if (p.split_off > 0) epi_tile_geglu<BN, false, true, true>(p, st, acc, t, wr, lane);
+          else epi_tile_geglu<BN, false, false, true>(p, st, acc, t, wr, lane);
+        } else if (p.split_off > 0) epi_tile_geglu<BN, false, true, false>(p, st, acc, t, wr, lane);
+        else if (nvalid == BM) epi_tile_geglu<BN, true, false, false>(p, st, acc, t, wr, lane);
+        else epi_tile_geglu<BN, false, false, false>(p, st, acc, t, wr, lane);
       }
-    } else if (!full) {
-      EpiRows R;
-      R.valid = 0;
-#pragma unroll
-      for (int i = 0; i < ES; ++i) {
-        const int rr = wr + 4 * i + rsub;
-        R.img[i] = n0 + rr / rpi;
-        R.row[i] = row_base + rr;
-        if (rr < nvalid) R.valid |= 1u << i;
-      }
-      if (p.fast_epi) epi_tile_generic<BN, true>(p, st, acc, R, tn, lane);
-      else epi_tile_generic<BN, false>(p, st, acc, R, tn, lane);
-    } else {
-      const long long r0 = row_base + wr + rsub;
-      const int img0 = n0 + (wr + rsub) / rpi;
-      const bool rv_uniform = (rpi % 16) == 0;   // the warp's 16 rows lie in one image
-      // image of this warp's 16 consecutive output rows for the GroupNorm statistics (stats_hw % 16 == 0: host check)
-      const long long simg = p.col_stats ? (row_base + wr) / p.stats_hw : 0;
+    } else if (p.fast_epi && p.ksplit == 1 && nvalid == BM && (w.tn + 1) * BN <= p.Ncols) {
       switch (mode) {
-        case 2: epi_tile_full<BN, false, true, false>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
-        case 3: epi_tile_full<BN, true, true, false>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
-        case 4: epi_tile_full<BN, false, false, true>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
-        case 5: epi_tile_full<BN, true, false, true>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
-        case 6: epi_tile_full<BN, false, true, true>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
-        default: epi_tile_full<BN, true, true, true>(p, st, acc, r0, img0, rv_uniform, tn, lane, simg); break;
+        case 2: epi_tile<BN, EPI_FULL, 2>(p, st, acc, t, wr, lane); break;
+        case 3: epi_tile<BN, EPI_FULL, 3>(p, st, acc, t, wr, lane); break;
+        case 4: epi_tile<BN, EPI_FULL, 4>(p, st, acc, t, wr, lane); break;
+        case 5: epi_tile<BN, EPI_FULL, 5>(p, st, acc, t, wr, lane); break;
+        case 6: epi_tile<BN, EPI_FULL, 6>(p, st, acc, t, wr, lane); break;
+        default: epi_tile<BN, EPI_FULL, 7>(p, st, acc, t, wr, lane); break;
       }
+    } else if (p.fast_epi) {
+      epi_tile<BN, EPI_VEC, 7>(p, st, acc, t, wr, lane);
+    } else {
+      epi_tile<BN, EPI_SCALAR, 7>(p, st, acc, t, wr, lane);
     }
   }
 }
@@ -683,11 +541,9 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
       bn_tile = 160;
       // under-filled launches (e.g. the 32x2 level of the UNet: 8 M tiles)
       if ((long long)p.m_tiles * (N / 160) * 2 <= num_sms()) {
-        static int splitk = -1;   // TNG_GEMM_SPLITK=0 disables (A/B measurements)
-        if (splitk < 0) { const char* e = getenv("TNG_GEMM_SPLITK"); splitk = e ? atoi(e) : 1; }
         long long kit = 0;
         for (int i = 0; i < d->n_groups; ++i) kit += d->g[i].nkb;
-        const bool can_split = splitk && d->out_f32 && !d->out_bf16 && !d->accumulate && d->act == TNG_ACT_NONE &&
+        const bool can_split = d->out_f32 && !d->out_bf16 && !d->accumulate && d->act == TNG_ACT_NONE &&
                                d->res != d->out_f32 && kit >= 32 && d->Ncols % 4 == 0;
         if (can_split) ksplit = 2;   // two CTAs per output tile, each reduces half of K (long reductions only)
         else if (N % 128 == 0 && (long long)p.m_tiles * (N / 128) <= num_sms()) bn_tile = 128;  // more, smaller N tiles
@@ -732,7 +588,6 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
   }
   if (d->out_f32 && (!al16(d->out_f32) || d->ld_f32 % 4)) vec = false;
   if (d->out_bf16 && (!al16(d->out_bf16) || d->ld_bf16 % 8 || d->split_off % 8)) vec = false;
-  p.vec_ok = vec ? 1 : 0;
   p.fast_epi = (vec && d->Ncols % 4 == 0) ? 1 : 0;
   if ((d->act == TNG_ACT_GEGLU || d->act == TNG_ACT_GEGLU_TANH) && !vec) return set_error(TNG_EINVAL, "GEGLU epilogue needs 16-byte aligned output");
   if (d->gn_stats) {
