@@ -6,7 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from tango_b200 import ops
-from test_kernel_contract_gpu import (NAN, SENT, U32, Out, attn_ref64, bf, coef_rows, el_err, excess,
+from test_kernel_contract_gpu import (NAN, SENT, U32, Out, attn_ref, bf, coef_rows, el_err, excess,
                                       flat_base, gemm_reference, group_fit, poisoned, poisoned_flat, rowcol_err,
                                       skip_concat, skip_concat_groups)
 
@@ -104,7 +104,7 @@ def test_attention_reference_matches_torch():
     q, k, v = (torch.randn(B * n, heads * 64, generator=g, dtype=torch.float64) for n in (Lq, Lk, Lk))
     kb = torch.zeros(B, Lk)
     kb[1, 4:] = -10000.0
-    o, pv = attn_ref64(q, k, v, batch=B, heads=heads, Lq=Lq, Lk=Lk, scale=0.125, kbias=kb)
+    o, pv = attn_ref(q, k, v, batch=B, heads=heads, Lq=Lq, Lk=Lk, scale=0.125, kbias=kb)
     sh = lambda t, n: t.view(B, n, heads, 64).transpose(1, 2)
     ref = F.scaled_dot_product_attention(sh(q, Lq), sh(k, Lk), sh(v, Lk), attn_mask=kb.double()[:, None, None, :],
                                          scale=0.125).transpose(1, 2).reshape(B * Lq, -1)

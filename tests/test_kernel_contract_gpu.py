@@ -452,17 +452,17 @@ def test_gemm_groupnorm_statistics_every_variant(cuda, case):
 
 
 # ---------------------------------------------------------------------------------------------------- tng_attention
-def attn_ref64(q, k, v, *, batch, heads, Lq, Lk, scale, kbias=None):
+def attn_ref(q, k, v, *, batch, heads, Lq, Lk, scale, kbias=None, width=64):
     """fp64 softmax(q k^T * scale + kbias) v and softmax |v| (the per-element scale of the P rounding error);
-    q / k / v: [rows, heads * 64] fp64."""
-    qh = q.view(batch, Lq, heads, 64).transpose(1, 2)
-    kh = k.view(batch, Lk, heads, 64).transpose(1, 2)
-    vh = v.view(batch, Lk, heads, 64).transpose(1, 2)
+    q / k / v: [rows, heads * width] fp64."""
+    qh = q.view(batch, Lq, heads, width).transpose(1, 2)
+    kh = k.view(batch, Lk, heads, width).transpose(1, 2)
+    vh = v.view(batch, Lk, heads, width).transpose(1, 2)
     s = qh @ kh.transpose(-1, -2) * scale
     if kbias is not None:
         s = s + kbias.double().view(batch, 1, 1, Lk)
     p = s.softmax(-1)
-    back = lambda t: t.transpose(1, 2).reshape(batch * Lq, heads * 64)
+    back = lambda t: t.transpose(1, 2).reshape(batch * Lq, heads * width)
     return back(p @ vh), back(p @ vh.abs())
 
 
@@ -519,7 +519,7 @@ def run_attention_case(cuda, B, heads, Lq, Lk, nsplit, kbias=None, seed=0, offse
     L.attention(qbuf, kvbuf, kvbuf, out.view, batch=B, heads=heads, Lq=Lq, Lk=Lk, scale=0.125, q_col0=qc, k_col0=kc,
                 v_col0=vc, kbias=kb_dev, nsplit=nsplit, split_off=split_off, **lo)
     torch.cuda.synchronize()
-    ref, pv = attn_ref64(qr, kr, vr, batch=B, heads=heads, Lq=Lq, Lk=Lk, scale=0.125, kbias=kbias)
+    ref, pv = attn_ref(qr, kr, vr, batch=B, heads=heads, Lq=Lq, Lk=Lk, scale=0.125, kbias=kbias)
     assert out.sentinel_intact()
     if nsplit == 1:
         # P enters the PV product rounded to bf16 (<= 2^-8 relative each, the normaliser keeps the fp32 values) and the
@@ -561,6 +561,27 @@ def test_attention_masking(cuda, mask):
     out, ref = run_attention_case(cuda, B, heads, Lq, Lk, 1, kbias=kb, seed=len(mask), offset=False)
     if mask == "all keys but one":   # the output rows are that key's value row (rounded to bf16)
         assert torch.equal(out.hi.cpu().view(B, Lq, -1)[0], bf(ref.view(B, Lq, -1)[0]).expand(Lq, -1))
+
+
+@pytest.mark.parametrize("L_,spread", [(128, 1.0), (384, 1.0), (384, 6.0)])
+def test_attention_wide_sliced_operands(cuda, L_, spread):
+    """tng_attention_wide (the VAE AttnBlock: one head of width 512) with B = 2, q / k / v at non-zero columns of one
+    NaN-padded fused buffer (ld > 3 * 512) and an output at a column offset with ld_o > 512: both 256-column halves land
+    in place and the padding stays untouched. `spread` > 1 makes the key magnitudes grow along the sequence so that the
+    running row maximum moves. Same per-element bound as the bf16 head-64 kernel."""
+    B, C = 2, 512
+    g = torch.Generator().manual_seed(L_ + int(spread))
+    q = bf(rand(g, B * L_, C))
+    k = bf(rand(g, B * L_, C) * torch.linspace(1.0, spread, L_).repeat(B)[:, None])
+    v = bf(rand(g, B * L_, C) + 0.5)
+    buf, (qc, kc, vc) = fused_buffer([q, k, v], cuda)
+    assert buf.stride(0) > 3 * C and min(qc, kc, vc) > 0
+    out = Out(B * L_, C, dtype=torch.bfloat16, device=cuda, col0=8, ld=C + 24)
+    L.attention_wide(buf, buf, buf, out.view, batch=B, L=L_, dim=C, scale=C ** -0.5, q_col0=qc, k_col0=kc, v_col0=vc)
+    torch.cuda.synchronize()
+    ref, pv = attn_ref(q.double(), k.double(), v.double(), batch=B, heads=1, Lq=L_, Lk=L_, scale=C ** -0.5, width=C)
+    assert out.sentinel_intact()
+    assert excess(out.hi, ref, 2.0 ** -7 * pv + 2.0 ** -8 * ref.abs()) <= 1.0
 
 
 # ---------------------------------------------------------------------------------------------------- tng_sched_step
