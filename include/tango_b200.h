@@ -248,6 +248,25 @@ int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guida
                  void* next_in, int64_t ld_in, int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Latent blend of text-guided editing / inpainting (one HBM pass), run after tng_sched_step / tng_dpm_step.
+ * Replaces: the schedulers' add_noise (scheduling_ddpm.py:351-372; DDIM and DPM-Solver use the same formula) and the
+ *           masking of StableDiffusionInpaintPipelineLegacy (pipeline_stable_diffusion_inpaint_legacy.py:692-709).
+ * coef = float[2] {sqrt(alphas_cumprod[t]), sqrt(1 - alphas_cumprod[t])} computed on the host in fp32 (device pointer).
+ *   p      = sqrt_a * x0 + sqrt_1ma * noise              (the noise term is dropped when noise == NULL)
+ *   sample = p                                           (mask == NULL: add_noise)
+ *   sample = p * m + sample * (1 - m)                    (mask: 1 keeps the noised input, 0 keeps sample)
+ * every product / sum is one round-to-nearest fp32 op (no fma), so the result equals the fork's CPU fp32 ops bit for
+ * bit; coef = {1, 0} with noise == NULL is the final blend x0 * m + sample * (1 - m). x0, noise, sample: fp32 NCHW
+ * [B, C, HW]; sample is read only under a mask and may not alias x0 or noise. mask: fp32 [Bm, HW], entry b at
+ * mask + b * mask_bstride (0 broadcasts one mask over the batch). Optionally also writes next_in: the channels-last
+ * bf16 UNet input [(2)B, HW, ld_in] (duplicated for the CFG halves when cfg, hi/lo split at split_off when > 0), as
+ * tng_sched_step packs it.
+ */
+int tng_latent_blend(const float* x0, const float* noise, const float* mask, int64_t mask_bstride, const float* coef,
+                     float* sample, void* next_in, int64_t ld_in, int32_t cfg, int32_t split_off, int64_t B, int64_t C,
+                     int64_t HW, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Small exact-fp32 pieces.
  * tng_timestep_embedding: get_timestep_embedding (embeddings.py:22-62), flip_sin_to_cos / freq_shift configurable.
  * tng_linear_f32: y = act(x) @ W^T + b for tiny M (TimestepEmbedding, resnet time_emb_proj; embeddings.py:200-212,

@@ -24,7 +24,7 @@ SYMBOLS = [
     "tng_groupnorm_stats", "tng_groupnorm_apply", "tng_layernorm", "tng_cast_act", "tng_softmax_rows",
     "tng_transpose_bf16", "tng_sched_step", "tng_timestep_embedding", "tng_linear_f32", "tng_convt_gather",
     "tng_tanh_to_i16", "tng_rmsnorm", "tng_gather_rows", "tng_rel_attention", "tng_stft_frames", "tng_stft_magnitude",
-    "tng_log_clamp", "tng_attention_wide", "tng_gemm_plan", "tng_dpm_step",
+    "tng_log_clamp", "tng_attention_wide", "tng_gemm_plan", "tng_dpm_step", "tng_latent_blend",
 ]
 
 
@@ -105,6 +105,7 @@ def load(build_if_missing: bool = True) -> C.CDLL:
         "tng_transpose_bf16": [vp, i64, i64, i64, i64, vp, i64, vp],
         "tng_sched_step": [vp, i64, i32, f32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
         "tng_dpm_step": [vp, i64, i32, f32, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
+        "tng_latent_blend": [vp, vp, vp, i64, vp, vp, vp, i64, i32, i32, i64, i64, i64, vp],
         "tng_timestep_embedding": [vp, i64, i32, i32, f32, vp, vp],
         "tng_linear_f32": [vp, i64, i64, vp, vp, i64, i32, i32, vp, vp],
         "tng_convt_gather": [vp, i64, i64, i32, i64, i32, i32, i64, vp, vp, vp],
@@ -404,6 +405,24 @@ def dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, ne
     _call("dpm_step", nbytes, load().tng_dpm_step, model_out.data_ptr(), model_out.stride(0), int(cfg), guidance,
           sample.data_ptr(), coef.data_ptr(), order, m0.data_ptr(), ptr(m1), ptr(m2), ptr(prev), ptr(next_in),
           0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
+
+
+def latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW, cfg=False, split_off=0):
+    """tng_latent_blend: sample = add_noise(x0, noise) (mask None) or add_noise(x0, noise) * m + sample * (1 - m);
+    noise None drops the noise term. mask: fp32 [Bm, HW] with Bm = 1 (broadcast) or B. Optionally packs the next UNet
+    input as sched_step does; see include/tango_b200.h."""
+    require_cuda(x0, noise, mask, coef, sample, next_in)
+    mstride = 0
+    if mask is not None:
+        if mask.dtype != torch.float32 or not mask.is_contiguous() or mask.numel() not in (HW, B * HW):
+            raise TangoB200Error(f"latent_blend: mask must be a contiguous fp32 [1 or {B}, {HW}] tensor")
+        mstride = 0 if mask.numel() == HW else HW
+    n = B * Cc * HW
+    nbytes = n * 4 * (1 + (noise is not None) + (mask is not None) + 1) + (0 if mask is None else mask.numel() * 4) \
+        + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
+    _call("latent_blend", nbytes, load().tng_latent_blend, x0.data_ptr(), ptr(noise), ptr(mask), mstride,
+          coef.data_ptr(), sample.data_ptr(), ptr(next_in), 0 if next_in is None else next_in.stride(0), int(cfg),
+          split_off, B, Cc, HW, stream_ptr())
 
 
 def timestep_embedding(t, dim, flip_sin_to_cos, freq_shift, out):

@@ -36,7 +36,7 @@ from . import parallel
 from . import synth
 from .blocks import GraphCache
 from .schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
-from .stft import TacotronSTFT
+from .stft import TacotronSTFT, wav_to_fbank
 from .t5 import T5EncoderModel
 from .unet import UNet2DConditionModel
 from .vae import AutoencoderKL
@@ -277,10 +277,13 @@ class AudioDiffusion:
         full = torch.randn((total,) + tuple(shape[1:]), generator=generator, device=gdev, dtype=dtype).to(device)
         return full if (lo == 0 and hi == total) else full[lo:hi].contiguous()
 
-    def advance_rng(self, total_batch, inference_scheduler, num_steps, generator=None, latent_shape=LATENT_HW):
+    def advance_rng(self, total_batch, inference_scheduler, num_steps, generator=None, latent_shape=LATENT_HW, *,
+                    edit_clips: Optional[int] = None, strength: float = 1.0):
         """Consume exactly the random numbers `inference` would for a `total_batch`-sample batch without running it:
         a rank whose shard of a chunk is empty calls this so that its (shared-seed) stream stays aligned with the
-        one-GPU run for the chunks that follow. Per-sample generator lists need nothing."""
+        one-GPU run for the chunks that follow. Per-sample generator lists need nothing. An edit (`edit_clips` input
+        clips in the chunk) draws the posterior noise of its clips, then the add-noise draw, then runs only the steps
+        that `strength` leaves."""
         if isinstance(generator, (list, tuple)) and len(generator) > 1:
             return
         if isinstance(generator, (list, tuple)):
@@ -289,8 +292,12 @@ class AudioDiffusion:
         sch.set_timesteps(num_steps, device=self.device)
         gdev = self.device if generator is None else generator.device
         shape = (total_batch, self.unet.config["in_channels"], *latent_shape)
+        t_start = 0
+        if edit_clips is not None:
+            t_start, _ = sch.get_timesteps(num_steps, strength)
+            torch.randn((edit_clips,) + shape[1:], generator=generator, device=gdev, dtype=torch.float32)
         torch.randn(shape, generator=generator, device=gdev, dtype=torch.float32)
-        for i in range(len(sch.timesteps)):
+        for i in range(t_start, len(sch.timesteps)):
             if sch._needs_noise(sch.timestep_at(i)):
                 torch.randn(shape, generator=generator, device=gdev, dtype=torch.float32)
 
@@ -307,14 +314,23 @@ class AudioDiffusion:
                   disable_progress=True, *, prompt_embeds: Optional[torch.Tensor] = None,
                   boolean_prompt_mask: Optional[torch.Tensor] = None, latents: Optional[torch.Tensor] = None,
                   noises: Optional[Sequence[torch.Tensor]] = None, generator=None, latent_shape=LATENT_HW,
-                  trace: Optional[list] = None, extra_streams=(), noise_rows=None) -> torch.Tensor:
+                  trace: Optional[list] = None, extra_streams=(), noise_rows=None,
+                  init_latents: Optional[torch.Tensor] = None, strength: float = 1.0,
+                  inpaint_mask: Optional[torch.Tensor] = None, init_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         """models.py:210-257. Extra keyword-only arguments (all optional): inject conditioning (`prompt_embeds`
         [(2)B, L, D] + `boolean_prompt_mask`), initial `latents`, per-step `noises` (one (B,8,H,W) tensor per step,
         used where the reference draws randn) or a torch `generator` (or a list with one generator per sample, as
         diffusers' randn_tensor accepts); `noise_rows` = (lo, hi, total) when this process holds samples [lo, hi) of a
         `total`-sample batch sharded over GPUs (see randn_rows); `latent_shape` for clips other than 10 s;
         `extra_streams` = ((encoded beats [(2)B, L, D], mask), (encoded chords, mask)) turns the loop into Mustango's
-        MusicAudioDiffusion.inference (mustango/models.py:540-600; needs a UNet config with the *Music blocks)."""
+        MusicAudioDiffusion.inference (mustango/models.py:540-600; needs a UNet config with the *Music blocks).
+
+        Editing (the loop of the fork's img2img / legacy-inpaint pipelines, DESIGN.md §9): `init_latents` are the clean
+        latents x0 [(B or 1), 8, H, W] of the input clip; the loop runs timesteps[t_start:] with t_start from `strength`
+        (`get_timesteps`) and starts from add_noise(x0, init_noise, timesteps[t_start]). `init_noise` (B, 8, H, W)
+        replaces that draw. With `inpaint_mask` [(B or 1), 1, H, W] in [0, 1] (1 keeps the input) every step is
+        followed by add_noise(x0, init_noise, t_i) * m + latents * (1 - m) and the loop by x0 * m + latents * (1 - m).
+        `noises[k]` then belongs to the k-th executed step."""
         device = self.device
         L.require_cuda_device(device)   # no CPU fallback
         cfg_on = guidance_scale > 1.0
@@ -332,12 +348,24 @@ class AudioDiffusion:
         timesteps = sch.timesteps
         Cl = self.unet.config["in_channels"]
         H, W = latent_shape
-        if latents is None:
+        edit = init_latents is not None
+        t_start, mask = 0, None
+        if edit:
+            if latents is not None:
+                raise ValueError("pass either `latents` (generation) or `init_latents` (editing), not both")
+            t_start, _ = sch.get_timesteps(num_steps, strength)
+            x0, edit_noise, mask = self._edit_inputs(init_latents, init_noise, inpaint_mask, batch_size, Cl, H, W,
+                                                     generator, noise_rows)
+            sample = torch.empty(batch_size, Cl, H, W, device=device, dtype=torch.float32)
+        elif inpaint_mask is not None or init_noise is not None or strength != 1.0:
+            raise ValueError("`strength`, `inpaint_mask` and `init_noise` need `init_latents`")
+        elif latents is None:
             latents = self.prepare_latents(batch_size, sch, Cl, torch.float32, device, generator, latent_shape,
                                            rows=noise_rows)
         else:
             latents = latents.to(device, torch.float32) * sch.init_noise_sigma
-        sample = latents.contiguous().clone()
+        if not edit:
+            sample = latents.contiguous().clone()
 
         unet = self.unet
         if boolean_prompt_mask is not None and prompt_embeds.shape[1] % self.LK_BUCKET:
@@ -354,7 +382,7 @@ class AudioDiffusion:
         if self._temb_cache.get("key") != tkey:   # batch- and data-independent: reuse across calls with the same grid
             self._temb_cache = {"key": tkey, "table": unet.time_embedding_table(timesteps)}
         temb_table = self._temb_cache["table"]                      # [steps, temb_total]
-        coef = sch.coefficient_table(device)                          # [steps, 10] (DPM-Solver: [steps, 11])
+        coef = sch.loop_table(device, t_start)                        # [steps, 10] (DPM-Solver: [steps, 11])
         s = unet.s
         HW = H * W
         # cfg_on is part of the key: the captured forward bakes in cfg_shared (the CFG shared prefix); so are the device
@@ -368,9 +396,15 @@ class AudioDiffusion:
             ident=torch.tensor([0, 0, 0, 1, 0, 0, 0, 0, 0, 1], device=device, dtype=torch.float32)))
         x_in, model_out, temb_cur = st.x_in, st.model_out, st.temb_cur
         so = Cl if unet.split else 0
-        # pack the initial latents into the (CFG-duplicated) channels-last bf16 UNet input
-        L.sched_step(None, cfg_on, float(guidance_scale), sample, None, st.ident, None, x_in, B=batch_size, Cc=Cl, HW=HW,
-                     split_off=so)
+        if edit:
+            # x_start = add_noise(x0, noise, timesteps[t_start]), packed into the UNet input in the same pass
+            blend = sch.blend_table(device)
+            L.latent_blend(x0, edit_noise, None, blend[t_start], sample, x_in, B=batch_size, Cc=Cl, HW=HW, cfg=cfg_on,
+                           split_off=so)
+        else:
+            # pack the initial latents into the (CFG-duplicated) channels-last bf16 UNet input
+            L.sched_step(None, cfg_on, float(guidance_scale), sample, None, st.ident, None, x_in, B=batch_size, Cc=Cl,
+                         HW=HW, split_off=so)
 
         def run_unet():
             unet.forward_rows(x_in, Bu, H, W, temb_cur, temb_cur.shape[1], out=model_out, cfg_shared=cfg_on)
@@ -388,7 +422,7 @@ class AudioDiffusion:
 
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-        for i in range(len(timesteps)):
+        for i in range(t_start, len(timesteps)):
             temb_cur.copy_(temb_table[i:i + 1].expand_as(temb_cur))
             if graph is not None:
                 graph.replay()
@@ -397,19 +431,51 @@ class AudioDiffusion:
             noise = None
             if sch._needs_noise(sch.timestep_at(i)):
                 if noises is not None:
-                    noise = noises[i].to(device, torch.float32).contiguous()
+                    noise = noises[i - t_start].to(device, torch.float32).contiguous()
                 else:
                     noise = self.randn_rows((batch_size, Cl, H, W), generator, device, torch.float32, noise_rows)
             sch._loop_step(i, model_out, cfg_on, float(guidance_scale), sample, noise, coef, x_in, st, B=batch_size,
                            Cc=Cl, HW=HW, split_off=so)
+            if mask is not None:
+                # inpaint_legacy:692-700: the kept region is the input noised to t_i, the step's start timestep
+                L.latent_blend(x0, edit_noise, mask, blend[i], sample, x_in, B=batch_size, Cc=Cl, HW=HW, cfg=cfg_on,
+                               split_off=so)
             if trace is not None:
                 trace.append(sample.clone())
+        if mask is not None:
+            # inpaint_legacy:709: x0 * m + latents * (1 - m) is the blend with coefficients (1, 0) and no noise term
+            keep = st.__dict__.setdefault("keep_row", torch.tensor([1.0, 0.0], device=device))
+            L.latent_blend(x0, None, mask, keep, sample, None, B=batch_size, Cc=Cl, HW=HW)
         ev1.record()
         torch.cuda.synchronize()
-        self.last_step_ms = ev0.elapsed_time(ev1) / max(1, len(timesteps))
+        n_run = len(timesteps) - t_start
+        self.last_step_ms = ev0.elapsed_time(ev1) / max(1, n_run)
         # kernels of libtango_b200.so executed by this call (graph replays re-run the captured launches)
-        self.last_kernel_launches = (L.launch_count() - n_eager0) + (per_forward * len(timesteps) if graph is not None else 0)
+        self.last_kernel_launches = (L.launch_count() - n_eager0) + (per_forward * n_run if graph is not None else 0)
         return sample
+
+    def _edit_inputs(self, init_latents, init_noise, inpaint_mask, batch_size, Cl, H, W, generator, noise_rows):
+        """x0, the add-noise draw (RNG draw 2 of the fork's order) and the [Bm, H*W] mask of an edit."""
+        device = self.device
+        x0 = torch.as_tensor(init_latents).to(device, torch.float32)
+        if x0.dim() != 4 or x0.shape[0] not in (1, batch_size) or tuple(x0.shape[1:]) != (Cl, H, W):
+            raise ValueError(f"init_latents must be ({batch_size} or 1, {Cl}, {H}, {W}), got {tuple(x0.shape)}")
+        x0 = x0.expand(batch_size, Cl, H, W).contiguous()
+        if init_noise is None:
+            noise = self.randn_rows((batch_size, Cl, H, W), generator, device, torch.float32, noise_rows)
+        else:
+            noise = torch.as_tensor(init_noise).to(device, torch.float32).contiguous()
+            if tuple(noise.shape) != (batch_size, Cl, H, W):
+                raise ValueError(f"init_noise must be ({batch_size}, {Cl}, {H}, {W}), got {tuple(noise.shape)}")
+        mask = None
+        if inpaint_mask is not None:
+            m = torch.as_tensor(inpaint_mask, dtype=torch.float32)
+            if m.dim() != 4 or m.shape[0] not in (1, batch_size) or tuple(m.shape[1:]) != (1, H, W):
+                raise ValueError(f"inpaint_mask must be ({batch_size} or 1, 1, {H}, {W}), got {tuple(m.shape)}")
+            if bool((m < 0).any()) or bool((m > 1).any()) or bool(torch.isnan(m).any()):
+                raise ValueError("inpaint_mask values must lie in [0, 1] (1 keeps the input, 0 regenerates)")
+            mask = m.reshape(m.shape[0], H * W).to(device).contiguous()
+        return x0, noise, mask
 
 
 class Tango:
@@ -461,7 +527,8 @@ class Tango:
                                                     "text_encoder_name": None}, device, precision, unet_config=ucfg,
                            allow_synthetic_tokenizer=True)
         self.model.unet.load_state_dict(synth.synth_state_dict(synth.unet_param_shapes(ucfg), seed))
-        self.vae.load_state_dict(synth.synth_state_dict(synth.vae_decoder_param_shapes(), seed))
+        self.vae.load_state_dict(synth.synth_state_dict(
+            dict(synth.vae_decoder_param_shapes(), **synth.vae_encoder_param_shapes()), seed))
         if scheduler == "ddim":
             self.scheduler = DDIMScheduler.from_pretrained(None)
         elif scheduler == "dpmsolver++":   # DPM-Solver++ 2M on the SD-2.1 betas (v-prediction)
@@ -500,9 +567,25 @@ class Tango:
         waveforms. The noise of a sharded run equals that of the one-GPU run on the same seed: each rank draws the
         chunk's full-batch tensors from its (identically seeded) generator and keeps its rows, or consumes only its own
         entries of a per-sample `generator` list (AudioDiffusion.randn_rows; diffusers torch_utils.py:29-70)."""
+        def run(k, batch, lo, hi, g, rows):
+            return self.model.inference(batch[lo:hi], self.scheduler, steps, guidance, samples,
+                                        disable_progress=disable_progress, generator=g, noise_rows=rows, **kw)
+
+        def skip(k, batch, g):
+            if kw.get("latents") is None and kw.get("noises") is None:
+                self.model.advance_rng(len(batch) * samples, self.scheduler, steps, g,
+                                       kw.get("latent_shape", LATENT_HW))
+
+        gens = kw.pop("generator", None)
+        return self._for_batch(prompts, samples, batch_size, shard, gens, run, skip)
+
+    def _for_batch(self, prompts, samples, batch_size, shard, gens, run, skip):
+        """Chunking, sharding and gathering of generate_for_batch / edit_for_batch. `run(k, batch, lo, hi, g, rows)`
+        returns the latents of prompts batch[lo:hi] of the chunk that starts at prompt k (`rows`: the sample rows of
+        this rank, see randn_rows); `skip(k, batch, g)` keeps the random stream aligned when this rank's shard of the
+        chunk is empty."""
         prompts = list(prompts)
         world, r = (parallel.world_size(), parallel.rank()) if shard else (1, 0)
-        gens = kw.pop("generator", None)
         per_sample = isinstance(gens, (list, tuple)) and len(gens) > 1
         if per_sample and len(gens) != len(prompts) * samples:
             raise ValueError(f"a per-sample generator list needs {len(prompts) * samples} entries, got {len(gens)}")
@@ -515,15 +598,124 @@ class Tango:
             if hi > lo:
                 rows = (lo * samples, hi * samples, len(batch) * samples) if world > 1 else None
                 with torch.no_grad():
-                    latents = self.model.inference(batch[lo:hi], self.scheduler, steps, guidance, samples,
-                                                   disable_progress=disable_progress, generator=g, noise_rows=rows, **kw)
-                    wave = self._decode(latents)
-            elif kw.get("latents") is None and kw.get("noises") is None:
-                self.model.advance_rng(len(batch) * samples, self.scheduler, steps, g,
-                                       kw.get("latent_shape", LATENT_HW))
+                    wave = self._decode(run(k, batch, lo, hi, g, rows))
+            else:
+                skip(k, batch, g)
             if world > 1:
                 wave = parallel.allgather_waves(wave, self.device)
             outputs += [item for item in wave]
         if samples == 1:
             return outputs
         return list(self.chunks(outputs, samples))
+
+    # ------------------------------------------------------------------------------------------ editing / inpainting
+    def edit(self, prompt, audio, strength=0.8, steps=100, guidance=3, samples=1, disable_progress=True, *,
+             time_mask_ratio_start_and_end=None, freq_mask_ratio_start_and_end=None, inpaint_mask=None, **kw):
+        """Re-render `audio` (a 16 kHz mono clip: numpy int16 or float array, or a torch tensor) under `prompt`.
+        `strength` in (0, 1] is how much of the denoising loop runs (0.8, the diffusers default, keeps little of the
+        input; small values stay close to it). Inpainting is an edit with a mask that regenerates only part of the clip:
+        `time_mask_ratio_start_and_end=(t0, t1)` regenerates the frames [t0, t1) of the clip's length and
+        `freq_mask_ratio_start_and_end=(f0, f1)` the mel bins [f0, f1) (AudioLDM's ratios), or `inpaint_mask`
+        (1 or B, 1, H, W) at latent resolution gives the mask itself (1 keeps the input, 0 regenerates). Returns the
+        int16 waveform (a list of `samples` waveforms when samples > 1)."""
+        return self.edit_for_batch([prompt], [audio], strength, steps, guidance, samples, batch_size=1,
+                                   disable_progress=disable_progress,
+                                   time_mask_ratio_start_and_end=time_mask_ratio_start_and_end,
+                                   freq_mask_ratio_start_and_end=freq_mask_ratio_start_and_end,
+                                   inpaint_mask=inpaint_mask, **kw)[0]
+
+    def edit_for_batch(self, prompts, audios, strength=0.8, steps=100, guidance=3, samples=1, batch_size=8,
+                       disable_progress=True, shard: bool = False, *, time_mask_ratio_start_and_end=None,
+                       freq_mask_ratio_start_and_end=None, inpaint_mask=None, **kw):
+        """`edit` for a list of prompts, chunked and sharded like generate_for_batch. `audios` is one clip that serves
+        every prompt or a list with one clip per prompt; `inpaint_mask` has one mask or one per prompt. Random numbers
+        are drawn in the fork pipelines' order: the posterior noise of the clips, the add-noise draw of the whole
+        batch, then one draw per executed DDPM step."""
+        prompts = list(prompts)
+        clips = [audios] if _is_one_clip(audios) else list(audios)
+        if len(clips) not in (1, len(prompts)):
+            raise ValueError(f"{len(clips)} clips for {len(prompts)} prompts: pass one clip or one per prompt")
+        clips = [_clip_tensor(c) for c in clips]
+        H, W = kw.pop("latent_shape", LATENT_HW)
+        if time_mask_ratio_start_and_end is not None or freq_mask_ratio_start_and_end is not None:
+            if inpaint_mask is not None:
+                raise ValueError("pass either mask ratios or `inpaint_mask`, not both")
+            inpaint_mask = ratio_mask(H, W, time_mask_ratio_start_and_end, freq_mask_ratio_start_and_end)
+        if inpaint_mask is not None:
+            inpaint_mask = torch.as_tensor(inpaint_mask, dtype=torch.float32)
+            if inpaint_mask.dim() != 4 or inpaint_mask.shape[0] not in (1, len(prompts)):
+                raise ValueError(f"inpaint_mask must be (1 or {len(prompts)}, 1, {H}, {W})")
+        if not self.vae.has_encoder:
+            raise L.TangoB200Error("editing needs the VAE encoder: the AutoencoderKL was loaded without encoder.* / "
+                                   "quant_conv.* weights")
+        self.scheduler.set_timesteps(steps)
+        self.scheduler.get_timesteps(steps, strength)      # refuses a strength that runs no step before any work
+        n_in = self.model.unet.config["in_channels"]
+
+        def run(k, batch, lo, hi, g, rows):
+            per_prompt = len(clips) > 1
+            mine = clips[k + lo:k + hi] if per_prompt else clips
+            crow = (lo, hi, len(batch)) if per_prompt and rows is not None else None
+            x0 = self._clip_latents(mine, (H, W), hi - lo, samples, g, crow, rows)
+            m = inpaint_mask
+            if m is not None and m.shape[0] > 1:
+                m = m[k + lo:k + hi].repeat_interleave(samples, 0)
+            return self.model.inference(batch[lo:hi], self.scheduler, steps, guidance, samples,
+                                        disable_progress=disable_progress, generator=g, noise_rows=rows,
+                                        latent_shape=(H, W), init_latents=x0, strength=strength, inpaint_mask=m, **kw)
+
+        def skip(k, batch, g):
+            if kw.get("init_noise") is None and kw.get("noises") is None:
+                self.model.advance_rng(len(batch) * samples, self.scheduler, steps, g, (H, W),
+                                       edit_clips=len(batch) if len(clips) > 1 else 1, strength=strength)
+
+        gens = kw.pop("generator", None)
+        return self._for_batch(prompts, samples, batch_size, shard, gens, run, skip)
+
+    def _clip_latents(self, clips, latent_shape, n_prompts, samples, generator, clip_rows, sample_rows):
+        """Clean latents x0 of `n_prompts * samples` edit samples (models.py:278-279 order: each prompt's samples are
+        adjacent): wav_to_fbank -> encode_first_stage -> get_first_stage_encoding. One generator draws the posterior
+        noise of the clips (rows `clip_rows` of the chunk's clips); a per-sample generator list draws each sample's
+        own, as the fork's img2img prepare_latents does."""
+        H, W = latent_shape
+        n_mel = self.stft.n_mel_channels
+        if W * 4 != n_mel:
+            raise ValueError(f"latent width {W} does not match the {n_mel} mel bins of the STFT (width {n_mel // 4})")
+        dev = self.device
+        fbank, _, _ = wav_to_fbank([c.to(dev) for c in clips], target_length=4 * H, fn_STFT=self.stft)
+        post = self.vae.encode_first_stage(fbank.unsqueeze(1).contiguous())
+        total = n_prompts * samples
+        if isinstance(generator, (list, tuple)) and len(generator) > 1:
+            idx = torch.arange(total, device=post.mean.device) // samples if len(clips) > 1 else \
+                torch.zeros(total, dtype=torch.long, device=post.mean.device)
+            mean, std = post.mean[idx], post.std[idx]
+            eps = self.model.randn_rows(tuple(mean.shape), generator, dev, torch.float32, sample_rows)
+            return self.vae.get_first_stage_encoding(mean + std * eps)
+        eps = self.model.randn_rows(tuple(post.mean.shape), generator, dev, torch.float32, clip_rows)
+        x0 = self.vae.get_first_stage_encoding(post.sample(noise=eps))
+        return x0.repeat_interleave(samples, 0) if len(clips) > 1 else x0.expand(total, *x0.shape[1:]).contiguous()
+
+
+def _is_one_clip(audio) -> bool:
+    return not isinstance(audio, (list, tuple)) and getattr(audio, "ndim", 1) == 1
+
+
+def _clip_tensor(audio) -> torch.Tensor:
+    """A 16 kHz mono clip as fp32: int16 PCM is scaled by 1/32768; float arrays and tensors are taken as they are."""
+    if isinstance(audio, np.ndarray) and audio.dtype == np.int16:
+        return torch.from_numpy(audio.astype(np.float32) / 32768.0)
+    t = torch.as_tensor(audio)
+    if t.dim() != 1 or t.numel() == 0:
+        raise ValueError(f"a clip must be a non-empty 1-D 16 kHz waveform, got shape {tuple(t.shape)}")
+    return t.float()
+
+
+def ratio_mask(H: int, W: int, time_ratio=None, freq_ratio=None) -> torch.Tensor:
+    """AudioLDM's inpainting mask at latent resolution (ldm.py:773-777): ones, with rows [int(H*t0):int(H*t1)] (time)
+    and columns [int(W*f0):int(W*f1)] (mel bins) zeroed for regeneration; (1.0, 1.0) is no band. (1, 1, H, W) fp32."""
+    t0, t1 = time_ratio if time_ratio is not None else (1.0, 1.0)
+    f0, f1 = freq_ratio if freq_ratio is not None else (1.0, 1.0)
+    m = torch.ones(1, 1, H, W)
+    m[:, :, int(H * t0):int(H * t1), :] = 0
+    m[:, :, :, int(W * f0):int(W * f1)] = 0
+    return m

@@ -130,6 +130,69 @@ class _SchedulerBase:
         """Row i of the coefficient table belongs to timesteps[i]."""
         return [self._coefficients(t) for t in self._t_list]
 
+    def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
+        """Coefficient table of a loop that runs timesteps[t_start:] (row i belongs to timesteps[i]); only the
+        multistep DPM-Solver's rows depend on where the loop starts."""
+        return self.coefficient_table(device)
+
+    def get_timesteps(self, num_inference_steps: int, strength: float):
+        """Img2img's `get_timesteps` (pipeline_stable_diffusion_img2img.py:509-516) on the grid of `set_timesteps`:
+        returns (t_start, timesteps[t_start:]). `strength` outside [0, 1], or so small that no step runs, raises."""
+        if strength < 0 or strength > 1:
+            raise ValueError(f"The value of strength should in [0.0, 1.0] but is {strength}")
+        init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
+        if init_timestep == 0:
+            raise ValueError(f"strength {strength} with {num_inference_steps} steps runs no denoising step "
+                             f"(int({num_inference_steps} * {strength}) == 0): raise the strength or the step count")
+        t_start = max(num_inference_steps - init_timestep, 0)
+        return t_start, self.timesteps[t_start:]
+
+    def _blend_row(self, t: int) -> torch.Tensor:
+        """add_noise's fp32 scalars at timestep t (scheduling_ddpm.py:361-366): alphas_cumprod[t] ** 0.5 and
+        (1 - alphas_cumprod[t]) ** 0.5."""
+        a = self.alphas_cumprod[torch.tensor([int(t)])]
+        return torch.cat([a ** 0.5, (1 - a) ** 0.5]).float()
+
+    def blend_table(self, device=None) -> torch.Tensor:
+        """[num_steps, 2] fp32 add_noise coefficients of the current grid (row i belongs to timesteps[i]): the
+        coefficient rows of tng_latent_blend."""
+        if self._coef_host is None:
+            self._finish_set_timesteps(None)
+        cache = self.__dict__.setdefault("_blend_cache", {})
+        key = tuple(self._t_list)
+        if key not in cache:
+            cache[key] = torch.stack([self._blend_row(t) for t in self._t_list]).contiguous()
+        tab = cache[key]
+        if device is None:
+            return tab
+        dkey = (key, str(torch.device(device)))
+        if dkey not in cache:
+            cache[dkey] = tab.to(device)
+        return cache[dkey]
+
+    def add_noise(self, original_samples: torch.Tensor, noise: torch.Tensor, timesteps) -> torch.Tensor:
+        """scheduling_ddpm.py:351-372 (DDIM and DPM-Solver share it) for fp32 CUDA tensors of shape (B, C, ...):
+        sqrt(alphas_cumprod[t]) * original_samples + sqrt(1 - alphas_cumprod[t]) * noise, on tng_latent_blend.
+        `timesteps` holds one timestep or one per sample."""
+        L.require_cuda(original_samples, noise)   # no CPU fallback
+        if original_samples.shape != noise.shape or original_samples.dim() < 2:
+            raise ValueError(f"add_noise: original_samples {tuple(original_samples.shape)} and noise "
+                             f"{tuple(noise.shape)} must share one (B, C, ...) shape")
+        ts = [int(t) for t in torch.as_tensor(timesteps).reshape(-1).tolist()]
+        B, Cc = original_samples.shape[:2]
+        if len(ts) not in (1, B):
+            raise ValueError(f"add_noise: {len(ts)} timesteps for a batch of {B}")
+        HW = original_samples[0, 0].numel()
+        x0, nz = original_samples.float().contiguous(), noise.float().contiguous()
+        out = torch.empty_like(x0)
+        rows = torch.stack([self._blend_row(t) for t in ts]).to(x0.device)
+        if len(ts) == 1:
+            L.latent_blend(x0, nz, None, rows[0], out, B=B, Cc=Cc, HW=HW)
+        else:
+            for b in range(B):
+                L.latent_blend(x0[b], nz[b], None, rows[b], out[b], B=1, Cc=Cc, HW=HW)
+        return out
+
     def _loop_step(self, i: int, model_out, cfg: bool, guidance: float, sample, noise, coef, next_in, bufs, *, B, Cc,
                    HW, split_off):
         """Step i of AudioDiffusion.inference: one fused CFG + update + next-UNet-input launch, `sample` updated in
@@ -345,6 +408,7 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         self.model_outputs = [None] * solver_order
         self.lower_order_nums = 0
         self._orders: list = []
+        self._loop_orders: list = []
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         """:185-206: linspace(0, T-1, n+1) rounded, reversed, last dropped (no steps_offset); resets the history."""
@@ -354,8 +418,8 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         self.timesteps = torch.from_numpy(ts)
         self.model_outputs = [None] * self.config["solver_order"]
         self.lower_order_nums = 0
-        n = len(ts)
-        self._orders = [self._order_at(i, n, min(i, self.config["solver_order"])) for i in range(n)]
+        self._orders = self._loop_orders_from(len(ts), 0)
+        self._loop_orders = self._orders
         self._finish_set_timesteps(device)
 
     def _needs_noise(self, t: int) -> bool:
@@ -370,6 +434,35 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         if cfg["solver_order"] == 2 or lower_order_nums < 2 or (low and i == n - 2):
             return 2
         return 3
+
+    def _loop_orders_from(self, n: int, t_start: int) -> list:
+        """Orders of a loop over steps t_start..n-1 of an n-step grid: the fork counts `lower_order_nums` from the
+        first `step` call, so the first executed step is order 1 and the next at most order 2, while the final-step
+        rules still look at the whole grid (:464-490). Entries before t_start are the full loop's."""
+        k = self.config["solver_order"]
+        full = [self._order_at(i, n, min(i, k)) for i in range(n)]
+        return full[:t_start] + [self._order_at(i, n, min(i - t_start, k)) for i in range(t_start, n)]
+
+    def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
+        """The coefficient table of a loop entered at timesteps[t_start] (an edit): its rows come from
+        `_coefficients_at` with the mid-grid orders, cached per (grid, t_start). t_start = 0 is the `set_timesteps`
+        table itself."""
+        if t_start == 0:
+            self._loop_orders = self._orders
+            return self.coefficient_table(device)
+        cache = self.__dict__.setdefault("_mid_cache", {})
+        key = (tuple(self._t_list), t_start)
+        if key not in cache:
+            orders = self._loop_orders_from(len(self._t_list), t_start)
+            rows = [self._coef_host[i] for i in range(t_start)] + \
+                [self._coefficients_at(i, orders[i]) for i in range(t_start, len(self._t_list))]
+            cache[key] = (orders, torch.stack(rows).contiguous(), {})
+        orders, host, dev = cache[key]
+        self._loop_orders = orders
+        d = str(torch.device(device))
+        if d not in dev:
+            dev[d] = host.to(device)
+        return dev[d]
 
     def order_at(self, i: int) -> int:
         """Order of step i in a loop started by `set_timesteps`."""
@@ -444,7 +537,7 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         """Step i of AudioDiffusion.inference: the converted output goes to slot i mod k of k = solver_order
         history slots, the previous ones are read from slots i-1 and i-2 mod k."""
         hist = self._history(bufs, sample)
-        k, order = self.config["solver_order"], self._orders[i]
+        k, order = self.config["solver_order"], self._loop_orders[i]
         m1 = hist[(i - 1) % k] if order >= 2 else None
         m2 = hist[(i - 2) % k] if order >= 3 else None
         L.dpm_step(model_out, cfg, guidance, sample, coef[i], order, hist[i % k], m1, m2, sample, next_in, B=B, Cc=Cc,

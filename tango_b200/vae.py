@@ -41,9 +41,11 @@ class DiagonalGaussianDistribution:
         if deterministic:
             self.var = self.std = torch.zeros_like(self.mean)
 
-    def sample(self, generator=None) -> torch.Tensor:
-        noise = torch.randn(self.mean.shape, generator=generator, device=self.mean.device, dtype=self.mean.dtype) \
-            if generator is not None else torch.randn(self.mean.shape).to(self.mean.device)
+    def sample(self, generator=None, noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """mean + std * noise; `noise` (of the mean's shape) replaces the draw."""
+        if noise is None:
+            noise = torch.randn(self.mean.shape, generator=generator, device=self.mean.device, dtype=self.mean.dtype) \
+                if generator is not None else torch.randn(self.mean.shape).to(self.mean.device)
         return self.mean + self.std * noise
 
     def mode(self) -> torch.Tensor:
@@ -365,6 +367,21 @@ class AutoencoderKL:
 
     def encode_first_stage(self, x: torch.Tensor) -> "DiagonalGaussianDistribution":
         return self.encode(x)
+
+    @property
+    def has_encoder(self) -> bool:
+        return self._esd is not None
+
+    def get_first_stage_encoding(self, encoder_posterior) -> torch.Tensor:
+        """autoencoder.py:126-135: scale_factor * (a sample of the posterior, or the given latents) — the latent space
+        the diffusion UNet was trained in."""
+        if isinstance(encoder_posterior, DiagonalGaussianDistribution):
+            z = encoder_posterior.sample()
+        elif isinstance(encoder_posterior, torch.Tensor):
+            z = encoder_posterior
+        else:
+            raise NotImplementedError(f"encoder_posterior of type '{type(encoder_posterior)}' not yet implemented")
+        return self.scale_factor * z
 
     # ------------------------------------------------------------------------------------------ vocoder
     def vocoder_rows(self, mel_rows: torch.Tensor, B: int, T: int):
