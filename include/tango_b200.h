@@ -26,7 +26,10 @@ extern "C" {
 #define TNG_ACT_NONE 0
 #define TNG_ACT_SILU 1
 #define TNG_ACT_LRELU 2 /* slope = act_param */
-#define TNG_ACT_GEGLU 3 /* out[j] = acc[j] * gelu_erf(acc[j + BN/2]) within each N tile (weights pre-interleaved) */
+/* out[j] = (acc[j] + bias[j]) * gelu_erf(acc[j + BN/2] + bias[j + BN/2]) within each N tile of BN columns (weights
+ * and bias pre-interleaved), written at output column tn * BN/2 + j. tng_conv_gemm only: BN = block_n (0 = auto) must be
+ * 128 or 256 and divide Ncols; bf16 output only (no out_f32, res or rowvec), 16-byte aligned, and alpha = 1. */
+#define TNG_ACT_GEGLU 3
 #define TNG_ACT_GEGLU_TANH 4 /* same pairing with the tanh-form GELU ("gelu_new": T5 v1.1 gated feed-forward) */
 
 #define TNG_DT_F32 0
@@ -270,7 +273,8 @@ int tng_latent_blend(const float* x0, const float* noise, const float* mask, int
  * Small exact-fp32 pieces.
  * tng_timestep_embedding: get_timestep_embedding (embeddings.py:22-62), flip_sin_to_cos / freq_shift configurable.
  * tng_linear_f32: y = act(x) @ W^T + b for tiny M (TimestepEmbedding, resnet time_emb_proj; embeddings.py:200-212,
- *                 resnet.py:572-573). pre_act is applied to x on load, post_act to y.
+ *                 resnet.py:572-573). pre_act is applied to x on load, post_act to y; each is TNG_ACT_NONE or
+ *                 TNG_ACT_SILU (anything else is TNG_EINVAL).
  */
 int tng_timestep_embedding(const float* t, int64_t n, int32_t dim, int32_t flip_sin_to_cos, float freq_shift,
                            float* out, void* stream);

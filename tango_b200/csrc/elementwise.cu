@@ -798,6 +798,8 @@ extern "C" int tng_timestep_embedding(const float* t, int64_t n, int32_t dim, in
 extern "C" int tng_linear_f32(const float* x, int64_t M, int64_t K, const float* w, const float* b, int64_t N,
                               int32_t pre_act, int32_t post_act, float* y, void* stream) {
   if (!x || !w || !y) return set_error(TNG_EINVAL, "linear_f32: null");
+  if ((pre_act != TNG_ACT_NONE && pre_act != TNG_ACT_SILU) || (post_act != TNG_ACT_NONE && post_act != TNG_ACT_SILU))
+    return set_error(TNG_EINVAL, "linear_f32: pre_act / post_act must be NONE or SILU (%d, %d)", pre_act, post_act);
   const long long threads = M * N * 32;
   linear_f32_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, ST(stream)>>>(x, M, (int)K, w, b, (int)N, pre_act, post_act, y);
   return check_launch("linear_f32");

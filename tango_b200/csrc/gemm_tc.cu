@@ -531,6 +531,8 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
     if ((bn_tile != 128 && bn_tile != 256) || d->Ncols % bn_tile != 0 || !d->out_bf16 || d->out_f32 || d->res ||
         d->rowvec)
       return set_error(TNG_EINVAL, "GEGLU epilogue needs block_n 128/256 dividing Ncols, bf16 output only");
+    // epi_tile_geglu applies the bias only: a scale would have to act on both halves before the GELU
+    if (d->alpha != 1.0f) return set_error(TNG_EINVAL, "GEGLU epilogue needs alpha = 1 (alpha=%g)", (double)d->alpha);
   }
   if (bn_tile == 0) {
     const long long N = d->Ncols;

@@ -77,6 +77,7 @@ def spec_conv_gemm(views, groups, weight, W, H, NB, *, bias=None, rowvec=None, r
         elif act in (ACT_GEGLU, ACT_GEGLU_TANH):
             bn = block_n
             assert bn in (128, 256) and Ncols % bn == 0
+            assert alpha == 1.0 and res is None and rowvec is None   # tng_conv_gemm: TNG_EINVAL otherwise
             t = z.view(rows, Ncols // bn, bn)
             gate = F.gelu(t[..., bn // 2:], approximate="tanh" if act == ACT_GEGLU_TANH else "none")
             z = (t[..., :bn // 2] * gate).reshape(rows, Ncols // 2)
@@ -278,7 +279,9 @@ def spec_stft_frames(y, pad, hi, lo):
 
 def spec_stft_magnitude(Fq, bins, mag_op, split_off, log_mag, energy, floor=1e-5):
     re, im = Fq[:, :bins].float(), Fq[:, bins:2 * bins].float()
-    m = torch.sqrt(re * re + im * im)
+    # IEEE sqrt of the fp32 sum (torch's vectorised fp32 sqrt on the CPU is not always correctly rounded; the fp64 root
+    # of an fp32 value rounds to the correctly rounded fp32 root)
+    m = torch.sqrt((re * re + im * im).double()).float()
     if mag_op is not None:
         _store_bf16(mag_op, m, split_off)
     if log_mag is not None:

@@ -44,3 +44,43 @@ def test_compute_call_fails_loudly_without_gpu():
     d.ld_f32 = 64
     rc = lib.tng_conv_gemm(ctypes.byref(d), None)
     assert rc != 0 and len(lib.tng_last_error()) > 0
+
+
+def _geglu_desc(buf, **kw):
+    """A valid GEGLU descriptor (2 N tiles of 256, bf16 output) over host memory: tng_gemm_plan never touches it."""
+    base = (ctypes.addressof(buf) + 255) // 256 * 256
+    d = L.GemmDesc()
+    d.n_aviews, d.n_groups, d.W, d.H, d.NB, d.Ncols, d.Ktot = 1, 1, 300, 1, 1, 512, 64
+    d.g[0] = L.KGroup(0, 0, 0, 0, 0, 1)
+    d.a[0] = L.AView(base, 64, 300, 1, 1, 64, 64 * 300, 64 * 300)
+    d.b, d.out_bf16, d.ld_bf16, d.act, d.alpha = base, base, 256, L.ACT_GEGLU, 1.0
+    for k, v in kw.items():
+        setattr(d, k, base if v is True else v)
+    return d
+
+
+def test_gemm_plan_rejects_unsupported_geglu_epilogues():
+    """The GEGLU epilogue applies the bias only: tng_gemm_plan (and so tng_conv_gemm) refuses alpha != 1, as it refuses a
+    residual, a row vector or an fp32 output; no device is needed to plan."""
+    lib = L.load()
+    buf = ctypes.create_string_buffer(1 << 16)
+    bn = ctypes.c_int32(0)
+    plan = lambda d: lib.tng_gemm_plan(ctypes.byref(d), ctypes.byref(bn), None, None)
+    for act in (L.ACT_GEGLU, L.ACT_GEGLU_TANH):
+        assert plan(_geglu_desc(buf, act=act)) == 0 and bn.value == 256
+        for bad in (dict(alpha=0.5), dict(alpha=3.0), dict(alpha=-1.0), dict(res=True, ldr=512), dict(rowvec=True),
+                    dict(out_f32=True, ld_f32=512), dict(block_n=64)):
+            assert plan(_geglu_desc(buf, act=act, **bad)) == -1, bad
+            assert b"GEGLU" in lib.tng_last_error()
+
+
+def test_linear_f32_rejects_activations_other_than_none_and_silu():
+    """tng_linear_f32 applies NONE or SILU only: every other activation id is TNG_EINVAL before any launch (LRELU would
+    run with a slope of 0, GEGLU as the identity)."""
+    lib = L.load()
+    x, w, y = (ctypes.create_string_buffer(4 * 64) for _ in range(3))
+    for pre, post in ((L.ACT_LRELU, L.ACT_NONE), (L.ACT_NONE, L.ACT_LRELU), (L.ACT_GEGLU, L.ACT_NONE),
+                      (L.ACT_NONE, L.ACT_GEGLU_TANH), (L.ACT_SILU, 5), (-1, L.ACT_SILU)):
+        rc = lib.tng_linear_f32(ctypes.addressof(x), 2, 8, ctypes.addressof(w), None, 4, pre, post, ctypes.addressof(y),
+                                None)
+        assert rc == -1 and b"linear_f32" in lib.tng_last_error(), (pre, post)

@@ -1,6 +1,7 @@
 """GPU: each C-ABI entry point against its `cabi_spec` statement (or an fp64 torch evaluation of the same bf16-rounded
 operands) at the descriptor features the host actually uses: sliced and offset operands, ld > C, ragged tails, several
-images per tile, scalar (misaligned / Ncols % 4 != 0) epilogues, hi/lo outputs, aliasing.
+images per tile, scalar (misaligned / Ncols % 4 != 0) epilogues, hi/lo outputs, aliasing; the GEGLU epilogue, the T5
+and mel front ends and the DPM-Solver step at the layouts the generate and edit paths use.
 
 Every input is a view into a larger buffer whose padding holds NaN, so a read past the logical extent poisons the result.
 Every output starts as NaN in its logical region (an element the kernel never writes fails) and as a finite sentinel
@@ -17,7 +18,8 @@ import torch.nn.functional as F
 import cabi_spec as S
 from tango_b200 import lib as L
 from tango_b200 import ops
-from tango_b200.schedulers import DDIMScheduler, DDPMScheduler
+from tango_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
+from test_dpm_solver_cpu import spec_dpm_step
 
 pytestmark = pytest.mark.gpu
 
@@ -451,6 +453,114 @@ def test_gemm_groupnorm_statistics_every_variant(cuda, case):
     assert excess(st[..., 1], (o * o).sum(1), bound * (o * o).sum(1)) <= 1.0
 
 
+# ---------------------------------------------------------------------------------------------------- GEGLU epilogue
+GELU_LIP = 1.13   # max |d gelu / dx| of both forms (1.129 at x ~ 1.41)
+
+
+def gelu64(x, tanh):
+    """fp64 GELU. The erf form through erfc and the tanh form as x * sigmoid(2u): neither cancels in the negative tail,
+    where 0.5 x (1 + tanh u) loses every digit (a 58 % "error" at x ~ -10)."""
+    x = x.double()
+    if tanh:
+        return x * torch.sigmoid(2.0 * math.sqrt(2.0 / math.pi) * (x + 0.044715 * x ** 3))
+    return 0.5 * x * torch.erfc(-x / math.sqrt(2.0))
+
+
+def geglu_halves(t, bn):
+    """[rows, Ncols] in the per-N-tile layout (BN/2 hidden columns, then their BN/2 gate columns) -> (hidden, gate),
+    each [rows, Ncols / 2] in output column order (tile tn at columns tn * BN/2)."""
+    v = t.double().reshape(t.shape[0], -1, bn)
+    return v[..., :bn // 2].reshape(t.shape[0], -1), v[..., bn // 2:].reshape(t.shape[0], -1)
+
+
+def geglu_reference(y, absdot, bn, tanh, *, gamma=GEMM_GAMMA):
+    """z = hidden * gelu(gate) in fp64 and its per-element allowance before the output rounding: gamma S_h |gelu(g)|
+    (summation error of the hidden half) + 1.13 |h| gamma S_g (of the gate half, through |gelu'| <= 1.13) + |h| |g| 2^-21
+    (the kernel's GELU: its formula is within 1.8e-7 |x| of the exact one, the ex2 / rcp approximations add <= 2^-22 |x|;
+    an absolute term, since the erf form's relative error reaches 1.6e-3 at x = -5). S_h / S_g: |operand| contractions."""
+    h, gt = geglu_halves(y, bn)
+    sh, sg = geglu_halves(absdot, bn)
+    gg = gelu64(gt, tanh)
+    return h * gg, gamma * sh * gg.abs() + GELU_LIP * h.abs() * gamma * sg + h.abs() * gt.abs() * 2.0 ** -21
+
+
+def geglu_weights(g, Ncols, bn, Cin):
+    """fp32 weight [Ncols, Cin] and bias for BN-column tiles whose second half is the gate: gate rows are halved and the
+    gate bias spreads over [-8.5, 8.5] in every tile, so the gates cover about [-9, 9] (both GELU tails); the hidden bias
+    is 1 + N(0, 0.5^2), so swapped halves cannot pass."""
+    gate = (torch.arange(Ncols) % bn) >= bn // 2
+    w = rand(g, Ncols, Cin, scale=Cin ** -0.5)
+    w[gate] *= 0.5
+    bias = 1.0 + 0.5 * rand(g, Ncols)
+    bias[gate] = torch.linspace(-8.5, 8.5, Ncols // 2)[torch.randperm(Ncols // 2, generator=g)]
+    return w, bias
+
+
+def geglu_operands(g, device, rows, bn, *, Cin=72):
+    """Two N tiles of a GEGLU GEMM: x bf16 [rows, Cin] (NaN-padded view), w bf16 [2 BN, Cin] in the kernel's per-tile
+    layout (NaN-padded view, ldb = 80 > Ktot = 72: the K block overhangs both), fp32 bias."""
+    w, bias = geglu_weights(g, 2 * bn, bn, Cin)
+    x = poisoned(bf(rand(g, rows, Cin)).to(device))
+    return x, poisoned(bf(w).to(device), col_pad=8, row_pad=0), bias.to(device)
+
+
+@pytest.mark.parametrize("split", [False, True])
+@pytest.mark.parametrize("rows", [256, 300])
+@pytest.mark.parametrize("bn", [128, 256])
+@pytest.mark.parametrize("tanh", [False, True])
+def test_geglu_epilogue_every_instantiation(cuda, tanh, bn, rows, split):
+    """Every epi_tile_geglu instantiation: {erf, tanh} x BN {128, 256} x {full tiles (256 rows), a ragged last tile (300
+    rows: 44 live)} x {bf16, hi/lo}, over two N tiles so that the second writes at output column BN/2. The output sits at
+    column 8 of a wider buffer (ld_bf16 > width, a gap before the lo half); everything around it keeps its sentinel."""
+    g = torch.Generator().manual_seed(bn + rows + 2 * split + 4 * tanh)
+    x, w, bias = geglu_operands(g, cuda, rows, bn)
+    views, groups = [row_view(x, 1, 1, rows)], k_groups_1x1(x.shape[1])
+    ob = Out(rows, bn, dtype=torch.bfloat16, device=cuda, col0=8, split_off=bn + 8 if split else 0, ld=2 * bn + 32)
+    L.conv_gemm(views, groups, w, rows, 1, 1, bias=bias, out_bf16=ob.view, act=L.ACT_GEGLU_TANH if tanh else L.ACT_GEGLU,
+                split_off=ob.split_off, block_n=bn)
+    torch.cuda.synchronize()
+    y, absdot = gemm_reference(views, groups, w, rows, 1, 1, bias=bias)
+    gate = geglu_halves(y, bn)[1]
+    assert gate.min() < -8 and gate.max() > 8
+    z, bound = geglu_reference(y, absdot, bn, tanh)
+    e = excess(ob.hi, z, bound + 2.0 ** -8 * z.abs())       # round to nearest bf16: half an ulp <= 2^-8 |z|
+    if split:                                                 # hi + lo carries z to 2^-17
+        e = max(e, excess(ob.value(), z, bound + 2.0 ** -16 * z.abs()))
+    print(f"geglu {'tanh' if tanh else 'erf'} BN={bn} rows={rows} {'hi/lo' if split else 'bf16'}: worst excess {e:.3f}")
+    assert e <= 1.0
+    assert ob.sentinel_intact()
+
+
+def geglu_linear_reference(x, wt, b, tanh, *, gamma):
+    """fp64 F.linear(x, wt, b).chunk(2) -> hidden * gelu(gate) (the diffusers / T5 GEGLU) with the geglu_reference
+    allowance: the whole output is one 'tile' of BN = Ncols."""
+    y = F.linear(x.double(), wt.double(), b.double())
+    absdot = F.linear(x.double().abs(), wt.double().abs(), b.double().abs())
+    return geglu_reference(y, absdot, wt.shape[0], tanh, gamma=gamma)
+
+
+@pytest.mark.parametrize("tanh", [False, True])
+def test_geglu_packed_conv_split(cuda, tanh):
+    """ops.PackedConv(geglu_bn=256) in split mode, as the UNet feed-forward (and T5 with the tanh form) packs it: the host
+    interleave of the hidden / gate rows and of the bias, hi/lo weights and operand, through tng_conv_gemm, against fp64
+    F.linear + hidden * gelu(gate) of the fp32 weights; 200 rows (ragged), inner = 256 (two N tiles). The 3-term split
+    products drop lo * lo (<= 2^-16 |x w| each with the lo rounding): gamma = 2 Gamma, as for the split convolutions."""
+    g = torch.Generator().manual_seed(11 + tanh)
+    rows, Cin, inner = 200, 128, 256
+    x = rand(g, rows, Cin)
+    wt, b = geglu_weights(g, 2 * inner, 2 * inner, Cin)
+    pc = ops.PackedConv(wt, b, split=True, device=cuda, geglu_bn=256, geglu_tanh=tanh)
+    xin = poisoned(torch.cat(pack_split(x), dim=1).to(cuda))
+    ob = Out(rows, inner, dtype=torch.bfloat16, device=cuda, split_off=inner, ld=2 * inner)
+    ops.run_linear(pc, xin, out_bf16=ob.view)
+    torch.cuda.synchronize()
+    z, bound = geglu_linear_reference(x, wt, b, tanh, gamma=2 * GEMM_GAMMA)
+    e = excess(ob.value(), z, bound + 2.0 ** -16 * z.abs())
+    print(f"geglu PackedConv split {'tanh' if tanh else 'erf'}: worst excess {e:.3f}")
+    assert e <= 1.0
+    assert ob.sentinel_intact()
+
+
 # ---------------------------------------------------------------------------------------------------- tng_attention
 def attn_ref(q, k, v, *, batch, heads, Lq, Lk, scale, kbias=None, width=64):
     """fp64 softmax(q k^T * scale + kbias) v and softmax |v| (the per-element scale of the P rounding error);
@@ -652,6 +762,65 @@ def test_sched_step_bit_exact(cuda, row, layout):
             assert (x0.abs() > c[8]).any()
 
 
+# ---------------------------------------------------------------------------------------------------- tng_dpm_step
+def dpm_rows():
+    """(name, order, row) from the product's own tables: the order 1, 2 and 3 rows (steps 0, 1 and 5 of a 20-step grid)
+    of a solver_order = 3 DPM-Solver++ and DPM-Solver, epsilon and v prediction."""
+    rows = []
+    for algo in ("dpmsolver++", "dpmsolver"):
+        for pred in ("epsilon", "v_prediction"):
+            s = DPMSolverMultistepScheduler(beta_schedule="scaled_linear", beta_start=0.00085, beta_end=0.012,
+                                            prediction_type=pred, algorithm_type=algo, solver_order=3)
+            s.set_timesteps(20)
+            tab = s.coefficient_table()
+            for i in (0, 1, 5):
+                rows.append((f"{algo}-{pred}", s.order_at(i), tab[i].clone()))
+    return rows
+
+
+@pytest.mark.parametrize("layout", ["cfg, hi/lo next_in, prev aliases sample",
+                                    "no cfg, plain next_in, separate prev",
+                                    "cfg, prev only",
+                                    "no cfg, hi/lo next_in only"])
+@pytest.mark.parametrize("row", range(12))
+def test_dpm_step_bit_exact(cuda, row, layout):
+    """tng_dpm_step equals spec_dpm_step bit for bit on order 1 / 2 / 3 rows of DPM-Solver(++) with epsilon and v
+    prediction: CFG or not, model_out with ld_mo > C (NaN padding), prev aliasing sample / separate / NULL, next_in plain
+    or hi/lo with a gap (compared over the whole buffer, sentinels included), history slots m1 / m2 NaN-padded past
+    B * C * HW = 888 (not a multiple of the 256-thread block), and m0 followed by a sentinel tail."""
+    name, order, coef = dpm_rows()[row]
+    B, Cc, HW = 3, 8, 37
+    n = B * Cc * HW
+    cfg = layout.startswith("cfg")
+    g = torch.Generator().manual_seed(row * 10 + len(layout))
+    mo = poisoned(rand(g, (2 if cfg else 1) * B * HW, Cc, scale=1.5).to(cuda), col_pad=8, align=4)
+    sample = rand(g, B, Cc, HW, scale=1.3).to(cuda)
+    m1 = poisoned_flat(rand(g, n).to(cuda)) if order >= 2 else None
+    m2 = poisoned_flat(rand(g, n).to(cuda)) if order == 3 else None
+    m0 = Out(1, n, dtype=torch.float32, device=cuda, ld=n, row_pad=1)
+    split = "hi/lo" in layout
+    nin = Out((2 if cfg else 1) * B * HW, Cc, dtype=torch.bfloat16, device=cuda, split_off=Cc + 8 if split else 0,
+              ld=2 * Cc + 16) if "next_in" in layout else None
+    alias = "aliases" in layout
+    prev = None if "next_in only" in layout else (sample if alias else torch.full((B, Cc, HW), NAN, device=cuda))
+    # the spec on CPU copies (same aliasing)
+    s_c = sample.cpu().clone()
+    p_c = None if prev is None else (s_c if alias else prev.cpu().clone())
+    m0_c = m0.cpu_clone()
+    n_c = None if nin is None else nin.cpu_clone()
+    spec_dpm_step(mo.cpu(), cfg, 3.0, s_c, coef, order, m0_c.buf[0], None if m1 is None else m1.cpu(),
+                  None if m2 is None else m2.cpu(), p_c, None if n_c is None else n_c.view, B=B, Cc=Cc, HW=HW,
+                  split_off=0 if nin is None else nin.split_off)
+    L.dpm_step(mo, cfg, 3.0, sample, poisoned_flat(coef.to(cuda), lead=4), order, m0.buf[0], m1, m2, prev,
+               None if nin is None else nin.view, B=B, Cc=Cc, HW=HW, split_off=0 if nin is None else nin.split_off)
+    torch.cuda.synchronize()
+    assert torch.equal(m0.buf.cpu(), m0_c.buf), name    # every element, the sentinel tail included
+    if prev is not None:
+        assert torch.equal(prev.cpu(), p_c), name
+    if nin is not None:
+        assert torch.equal(nin.buf.cpu(), n_c.buf), name
+
+
 # ---------------------------------------------------------------------------------------------------- GroupNorm
 def group_fit(got, ref, NB, HW, groups):
     """Per (image, group) least-squares fit got ~ a * ref + b (gamma = 1, beta = 0, so ref is the normalised value):
@@ -782,6 +951,127 @@ def test_layernorm_rmsnorm_template_boundaries(cuda, Cc):
     assert yr.sentinel_intact() and yf.sentinel_intact()
 
 
+# ---------------------------------------------------------------------------------------------------- T5 front end
+def test_gather_rows_ids_edges(cuda):
+    """tng_gather_rows bit for bit: ids 0, n - 1 and repeats, 21 rows (not a multiple of the 8 rows per CTA), the table
+    between NaN rows (a wrong row index reads NaN) and the rows past the output's end kept at the sentinel."""
+    g = torch.Generator().manual_seed(21)
+    n, C, rows = 50, 36, 21
+    tb = torch.full((n + 2, C), NAN)
+    tb[1:n + 1] = rand(g, n, C)
+    table = tb.to(cuda)[1:n + 1]
+    ids = torch.tensor([0, n - 1, 7, 7, 0, n - 1] + torch.randint(0, n, (rows - 6,), generator=g).tolist())
+    out = Out(rows, C, dtype=torch.float32, device=cuda, ld=C, row_pad=3)
+    L.gather_rows(table, ids.to(cuda), out.buf[:rows])
+    torch.cuda.synchronize()
+    assert torch.equal(out.hi.cpu(), table.cpu()[ids])
+    assert out.sentinel_intact()
+
+
+FMIN = torch.finfo(torch.float32).min   # the T5 extended attention mask value
+
+
+def rel_attn_ref(q, k, v, relbias, kbias, *, batch, heads, L):
+    """fp64 T5 self-attention softmax(q k^T + relbias[h, key - query + L - 1] + kbias[b, key]) v (no scaling) of
+    q / k / v [batch * L, heads * 64]. Also returns sum p |v| and the per-query score allowance: max over the live keys
+    of 2^-24 (64 sum_d |q_d k_d| + 4 |s|) (the fp32 fma chain over 64 dims, the bias add and s - max)."""
+    sh = lambda t: t.double().reshape(batch, L, heads, 64).transpose(1, 2)
+    qh, kh, vh = sh(q), sh(k), sh(v)
+    pos = torch.arange(L)
+    s = qh @ kh.transpose(-1, -2) + relbias.double()[:, pos[None, :] - pos[:, None] + L - 1][None]
+    live = torch.ones(batch, 1, 1, L, dtype=torch.bool)
+    if kbias is not None:
+        s = s + kbias.double().view(batch, 1, 1, L)
+        live = kbias.view(batch, 1, 1, L) > FMIN
+    p = s.softmax(-1)
+    ds = U32 * (64 * (qh.abs() @ kh.abs().transpose(-1, -2)) + 4 * s.abs())
+    ds = ds.masked_fill(~live, 0.0).amax(-1, keepdim=True).expand(-1, -1, -1, 64)
+    back = lambda t: t.transpose(1, 2).reshape(batch * L, heads * 64)
+    return back(p @ vh), back(p @ vh.abs()), back(ds)
+
+
+def rel_attn_bound(pv, ds, L_):
+    """A score error d moves the output by <= 2 d sum p |v|. The softmax arithmetic (u = 2^-24): the PV fma chain runs
+    over all L keys (L u), l takes 8 roundings per 64-key tile (pair sum, 5 butterfly steps, rescale, add), o one
+    rescale per tile, expf 2 ulp (4 u), 1 / l and the final product 2 u: (L + 9 ceil(L / 64) + 6) u <= 2 (L + 70) u of
+    sum p |v| for every L."""
+    return (2 * ds + 2 * (L_ + 70) * U32) * pv
+
+
+def rel_attn_operands(g, B, heads, L_, *, grow=False):
+    """q / k / v fp32 [B * L, heads * 64] and a relative bias [heads, 2L - 1] with a large, asymmetric spread (it rises
+    from -6 to +3 with key - query, plus N(0, 2^2)): a query - key index instead of key - query changes every row.
+    grow: key magnitudes rise 0.2 -> 2.5 along the sequence, so the running maximum moves in later key tiles."""
+    inner = heads * 64
+    q, k, v = (rand(g, B * L_, inner, scale=0.5) for _ in range(3))
+    v += 0.3
+    if grow:
+        k *= torch.linspace(0.2, 2.5, L_).repeat(B)[:, None]
+    relbias = rand(g, heads, 2 * L_ - 1, scale=2.0) + torch.linspace(-6.0, 3.0, 2 * L_ - 1)
+    return q, k, v, relbias
+
+
+def rel_attn_kbias(B, L_, mode):
+    """None, or an additive key mask of 0 / finfo.min: 'tail' masks the last b + 1 keys of sequence b, 'all but key 0'
+    every key but the first, 'one sequence' every key of sequence 1 (and a tail of sequence 0)."""
+    if mode is None:
+        return None
+    kb = torch.zeros(B, L_)
+    if mode == "tail":
+        for b in range(B):
+            kb[b, L_ - b - 1:] = FMIN
+    elif mode == "all but key 0":
+        kb[:, 1:] = FMIN
+    else:
+        kb[0, L_ - 3:] = FMIN
+        kb[1, :] = FMIN
+    return kb
+
+
+REL_CASES = [(1, 1, 1, None, True, False), (3, 2, 5, "tail", False, False), (2, 16, 16, None, True, False),
+             (3, 1, 17, "all but key 0", True, False), (2, 2, 64, "tail", True, False),
+             (3, 16, 65, "one sequence", False, False), (2, 2, 129, None, True, True),
+             (3, 1, 129, "one sequence", True, True)]
+
+
+@pytest.mark.parametrize("B,heads,L_,mask,split,grow", REL_CASES)
+def test_rel_attention_sequence_edges(cuda, B, heads, L_, mask, split, grow):
+    """tng_rel_attention at L = 1, 5, 16, 17, 64, 65, 129 (the 16-query CTA, 4 queries per warp, 64-key tiles) with
+    heads 1 / 2 / 16: q / k / v at non-zero, out-of-order columns (v, k, q) of one NaN-padded fp32 buffer with
+    ld > 3 * inner, relbias and kbias inside NaN padding, an output at a column offset (bf16, or hi/lo with a gap).
+    Against fp64 on the fp32 operands, per element. A fully masked sequence: every score absorbs into finfo.min alike
+    (in fp32 and in fp64), so its rows are the uniform mean of V."""
+    g = torch.Generator().manual_seed(B * 1000 + heads * 10 + L_)
+    inner = heads * 64
+    q, k, v, relbias = rel_attn_operands(g, B, heads, L_, grow=grow)
+    kb = rel_attn_kbias(B, L_, mask)
+    cols = {"v": 8, "k": 8 + inner + 4, "q": 8 + 2 * inner + 12}
+    buf = torch.full((B * L_ + 3, 3 * inner + 32), NAN)
+    for name, t in (("q", q), ("k", k), ("v", v)):
+        buf[:B * L_, cols[name]:cols[name] + inner] = t
+    qkv = buf.to(cuda)[:B * L_]
+    out = Out(B * L_, inner, dtype=torch.bfloat16, device=cuda, col0=4, split_off=inner + 8 if split else 0,
+              ld=2 * inner + 24)
+    L.rel_attention(qkv, poisoned_flat(relbias.reshape(-1).to(cuda), lead=3),
+                    None if kb is None else poisoned_flat(kb.reshape(-1).to(cuda), lead=1), out.view, batch=B,
+                    heads=heads, L=L_, q_col0=cols["q"], k_col0=cols["k"], v_col0=cols["v"], split_off=out.split_off)
+    torch.cuda.synchronize()
+    ref, pv, ds = rel_attn_ref(q, k, v, relbias, kb, batch=B, heads=heads, L=L_)
+    bound = rel_attn_bound(pv, ds, L_)
+    e = excess(out.hi, ref, bound + 2.0 ** -8 * ref.abs())
+    if split:
+        e = max(e, excess(out.value(), ref, bound + 2.0 ** -16 * ref.abs()))
+    print(f"rel_attention B={B} heads={heads} L={L_} mask={mask} {'hi/lo' if split else 'bf16'}: worst excess {e:.3f}")
+    assert e <= 1.0
+    assert out.sentinel_intact()
+    if mask == "one sequence":
+        mean_v = v.double().view(B, L_, inner)[1].mean(0)
+        assert el_err(ref.view(B, L_, inner)[1], mean_v.expand(L_, -1)) < 1e-12
+    if mask == "all but key 0":          # p = (1, 0, ...) exactly: the rows are key 0's value row
+        want = bf(v.view(B, L_, inner)[:, :1].expand(B, L_, inner).reshape(B * L_, inner))
+        assert torch.equal(out.hi.cpu(), want)
+
+
 # ---------------------------------------------------------------------------------------------------- small kernels
 def test_cast_act_upsample_hi_lo_ld(cuda):
     """tng_cast_act with ld_x > C, nearest x2 upsample, leaky-ReLU and a hi/lo output with a gap: bit for bit."""
@@ -892,3 +1182,147 @@ def test_timestep_embedding_odd_dim_freq_shift(cuda, dim, flip):
     if dim % 2:
         assert (out.hi[:, -1] == 0).all()
     assert out.sentinel_intact()
+
+
+# ---------------------------------------------------------------------------------------------------- tng_linear_f32
+def silu64(x):
+    return x * torch.sigmoid(x)
+
+
+def linear_f32_reference(x, w, b, pre, post):
+    """fp64 post(pre(x) w^T + b) and its per-element allowance (u = 2^-24): each lane sums ceil(K/32) products in one fma
+    chain, then 5 butterfly steps and the bias add: (ceil(K/32) + 6) u sum |a w| (+ |b|). The sm_90 SiLU (ex2 2 ulp, rcp
+    1 ulp, two roundings, and the rounding of its exponent argument: |x| u) is within (8 + |x|) u relative; |silu'| <= 1.1."""
+    x, w = x.double(), w.double()
+    bd = 0.0 if b is None else b.double()
+    a = silu64(x) if pre == L.ACT_SILU else x
+    y = a @ w.t() + bd
+    err = (math.ceil(x.shape[1] / 32) + 6) * U32 * (a.abs() @ w.abs().t() + abs(bd))
+    if pre == L.ACT_SILU:
+        err = err + U32 * (((8 + x.abs()) * a.abs()) @ w.abs().t())
+    if post == L.ACT_SILU:
+        z = silu64(y)
+        return z, 1.1 * err + U32 * (8 + y.abs()) * z.abs()
+    return y, err
+
+
+def linear_f32_operands(g, device, M, K, N, has_b):
+    """x [M, K], w [N, K] (dense, followed by NaN) and b [N] (inside NaN padding) or None."""
+    x = poisoned_flat(rand(g, M * K, scale=2.0).to(device)).view(M, K)
+    w = poisoned_flat(rand(g, N * K, scale=K ** -0.5).to(device)).view(N, K)
+    return x, w, poisoned_flat(rand(g, N).to(device), lead=2) if has_b else None
+
+
+@pytest.mark.parametrize("pre,post", [(L.ACT_NONE, L.ACT_NONE), (L.ACT_NONE, L.ACT_SILU), (L.ACT_SILU, L.ACT_NONE),
+                                      (L.ACT_SILU, L.ACT_SILU)])
+def test_linear_f32_shapes_and_activations(cuda, pre, post):
+    """tng_linear_f32 over M in {1, 5}, K in {31, 32, 320} (a partial lane stride, one stride, ten), N in {1, 7, 1280},
+    with and without a bias: per element against fp64, the rows past M kept at the sentinel."""
+    g = torch.Generator().manual_seed(pre * 2 + post)
+    worst = 0.0
+    for M in (1, 5):
+        for K in (31, 32, 320):
+            for N in (1, 7, 1280):
+                for has_b in (False, True):
+                    x, w, b = linear_f32_operands(g, cuda, M, K, N, has_b)
+                    y = Out(M, N, dtype=torch.float32, device=cuda, ld=N, row_pad=2)
+                    L.linear_f32(x, w, b, y.buf[:M], pre_act=pre, post_act=post)
+                    torch.cuda.synchronize()
+                    ref, bound = linear_f32_reference(x.cpu(), w.cpu(), None if b is None else b.cpu(), pre, post)
+                    e = excess(y.hi, ref, bound)
+                    worst = max(worst, e)
+                    assert e <= 1.0 and y.sentinel_intact(), (M, K, N, has_b, e)
+    print(f"linear_f32 pre={pre} post={post}: worst excess {worst:.3f}")
+
+
+# ---------------------------------------------------------------------------------------------------- mel front end
+FLOOR = 1e-5
+
+
+def ulp32(r):
+    """The fp32 ulp at each value of r (as fp64)."""
+    a = r.float().abs()
+    return (torch.nextafter(a, torch.tensor(math.inf)) - a).double()
+
+
+@pytest.mark.parametrize("pad,T", [(64, 65), (64, 131), (512, 513), (512, 1027)])
+def test_stft_frames_reflect_edges(cuda, pad, T):
+    """tng_stft_frames bit for bit against spec_stft_frames at T = pad + 1 (the shortest legal reflect) and T = 2 pad + 3,
+    B = 3, ld = T + 2 pad + 13: both planes entirely (the zero tail past T + 2 pad is written), rows past B untouched;
+    the waveform is followed by NaN."""
+    g = torch.Generator().manual_seed(pad + T)
+    B, ld = 3, T + 2 * pad + 13
+    y = poisoned_flat(rand(g, B * T, scale=0.5).to(cuda)).view(B, T)
+    hi, lo = (Out(B, ld, dtype=torch.bfloat16, device=cuda, ld=ld, row_pad=2) for _ in range(2))
+    hc, lc = hi.cpu_clone(), lo.cpu_clone()
+    S.spec_stft_frames(y.cpu(), pad, hc.buf[:B], lc.buf[:B])
+    L.stft_frames(y, pad, hi.buf[:B], lo.buf[:B])
+    torch.cuda.synchronize()
+    assert torch.equal(hi.buf.cpu(), hc.buf) and torch.equal(lo.buf.cpu(), lc.buf)
+    assert (hc.buf[:B, T + 2 * pad:] == 0).all() and (lc.buf[:B, T + 2 * pad:] == 0).all()
+
+
+@pytest.mark.parametrize("null_out", ["mag", "log_mag", "energy"])
+@pytest.mark.parametrize("bins", [17, 32, 33, 513])
+def test_stft_magnitude_layout_and_bounds(cuda, bins, null_out):
+    """tng_stft_magnitude with ldF > 2 bins (NaN past column 2 bins), 13 rows (not a multiple of the 8 warps), all-zero
+    frames and frames below the floor, each output NULL in turn. The magnitude is sqrt(rn(rn(re^2) + rn(im^2))), one IEEE
+    op per step on both sides: the operand is bit-exact against spec_stft_magnitude in the model's layout (hi at column 0,
+    lo at c_pad > bins; the pad columns [bins, c_pad) keep their sentinel: the mel GEMM reads them against zero weights).
+    log_mag within 1 ulp of the fp64 log (CUDA's documented logf bound); energy: an fma chain of ceil(bins / 32) per lane
+    and 5 butterfly steps, halved by the square root, + its rounding: ((ceil(bins/32) + 6) / 2 + 1) 2^-24 relative."""
+    g = torch.Generator().manual_seed(bins * 3 + len(null_out))
+    rows = 13
+    c_pad = (bins + 1 + 7) // 8 * 8
+    Fq = rand(g, rows, 2 * bins, scale=3.0)
+    Fq[[2, 9]] = 0.0                   # silent frames: log(floor)
+    Fq[5] *= 1e-7                      # below the floor
+    Fd = poisoned(Fq.to(cuda), col_pad=5, align=1)
+    mag = None if null_out == "mag" else Out(rows, bins, dtype=torch.bfloat16, device=cuda, split_off=c_pad,
+                                             ld=2 * c_pad + 8)
+    logm = None if null_out == "log_mag" else Out(rows, bins, dtype=torch.float32, device=cuda, ld=bins, row_pad=2)
+    en = None if null_out == "energy" else Out(rows, 1, dtype=torch.float32, device=cuda, ld=1, row_pad=3)
+    L.stft_magnitude(Fd, bins, None if mag is None else mag.view, c_pad, None if logm is None else logm.buf[:rows],
+                     None if en is None else en.buf[:rows, 0], FLOOR)
+    torch.cuda.synchronize()
+    m = torch.sqrt((Fq[:, :bins] * Fq[:, :bins] + Fq[:, bins:] * Fq[:, bins:]).double()).float()   # as the spec
+    if mag is not None:
+        mc = mag.cpu_clone()
+        S.spec_stft_magnitude(Fd.cpu(), bins, mc.view, c_pad, None, None, FLOOR)
+        assert torch.equal(mag.buf.cpu(), mc.buf)
+    msg = [f"stft_magnitude bins={bins} ({null_out} NULL):"]
+    if logm is not None:
+        ref = torch.log(torch.clamp(m.double(), min=torch.tensor(FLOOR, dtype=torch.float32).item()))
+        e = excess(logm.hi, ref, ulp32(ref))
+        msg.append(f"log_mag worst excess {e:.3f}")
+        assert e <= 1.0 and logm.sentinel_intact()
+        silent = logm.hi[[2, 9]].cpu()
+        assert (silent == silent[0, 0]).all()       # the same log(floor) everywhere
+    if en is not None:
+        ref = m.double().pow(2).sum(1).sqrt()
+        e = excess(en.hi[:, 0], ref, ((math.ceil(bins / 32) + 6) / 2 + 1) * U32 * ref + 1e-45)
+        msg.append(f"energy worst excess {e:.3f}")
+        assert e <= 1.0 and en.sentinel_intact()
+    print(" ".join(msg))
+
+
+def test_log_clamp_edges(cuda):
+    """tng_log_clamp on values below, at and just above the floor, 0, -0, negatives, denormals, +inf and a spread of
+    magnitudes; n = 1037 (not a multiple of 256) with a sentinel tail: every result within 1 ulp of the fp64
+    log(max(x, floor)), +inf to +inf."""
+    fl = torch.tensor(FLOOR, dtype=torch.float32)
+    special = torch.cat([torch.tensor([0.0, -0.0, -1.0, -1e30, 1e-45, 1e-40, 1.2e-38, 1.0, 2.5, 1e30, math.inf]),
+                         (fl * 0.999).view(1), fl.view(1), torch.nextafter(fl, torch.tensor(1.0)).view(1)])
+    g = torch.Generator().manual_seed(5)
+    x = torch.cat([special, torch.exp(rand(g, 1037 - special.numel(), scale=8.0))]).float()
+    n = x.numel()
+    y = Out(1, n, dtype=torch.float32, device=cuda, ld=n, row_pad=1)
+    L.log_clamp(poisoned_flat(x.to(cuda)), y.buf[0], FLOOR)
+    torch.cuda.synchronize()
+    ref = torch.log(torch.clamp(x.double(), min=fl.item()))
+    got = y.hi[0].cpu()
+    fin = torch.isfinite(ref)
+    e = excess(got[fin], ref[fin], ulp32(ref[fin]))
+    print(f"log_clamp: worst excess {e:.3f}")
+    assert e <= 1.0 and (got[~fin] == math.inf).all() and int((~fin).sum()) == 1
+    assert y.sentinel_intact()
