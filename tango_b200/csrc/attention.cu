@@ -2,20 +2,27 @@
 // VAE AttnBlock (audioldm/variational_autoencoder/modules.py:204-230: ONE head of width 512 over the H*W positions of
 // an image, 4096 positions for a 10 s clip, 12288 for 30 s). The score matrix never leaves the SM.
 //
-// One CTA = 128 query rows x DV value / output columns of one batch entry, 256 threads: warpgroup g owns query rows
+// One CTA = 128 query rows x DV value / output columns of one batch entry: consumer warpgroup g owns query rows
 // [64g, 64g + 64). Q / K / V arrive as TMA SWIZZLE_128B chunks of 64 columns (Q once; K / V in tiles of 64 keys, NBUF
-// buffers deep). Per key tile: S = Q K^T over the D/64 head chunks (wgmma m64n64k16, both operands K-major in shared
-// memory) -> fp32 online softmax in registers (the four lanes that share a row combine their maxima / sums by shuffles)
+// buffers deep). With NBUF > 1 a ninth warp (288 threads) is the producer: one of its lanes issues every load and
+// refills a K / V buffer as soon as both warpgroups have released it, so the consumers only wait for data and the
+// warpgroups can drift up to NBUF - 1 tiles apart (one's softmax then runs while the other's wgmma keep the tensor
+// cores busy).
+// Per key tile: S = Q K^T over the D/64 head chunks (wgmma m64n64k16, both operands K-major in shared memory)
+// -> fp32 online softmax in registers (the four lanes that share a row combine their maxima / sums by shuffles)
 // -> O += P V with P taken straight from registers as the A operand (the accumulator layout of S is the A-fragment
 // layout) and V consumed as an MN-major B operand (no transpose), 64 output columns per instruction.
 //
-//   <64, 64, 1, 3>    head width 64, bf16 operands: 64 KB of shared memory, two CTAs per SM.
+//   <64, 64, 1, 3>    head width 64, bf16 operands: 64 KB of shared memory, two CTAs per SM. 18 warps put 5 on one
+//                     SM sub-partition, whose 16 K registers leave 96 per thread; the consumers fit without spills.
 //   <64, 64, 2, 3>    the parity mode: every operand carries its bf16 rounding residual and each product is evaluated as
 //                     hi*hi + lo*hi + hi*lo, which restores ~fp32 accuracy on the bf16 tensor cores (1 CTA / SM).
 //   <512, 256, 1, 1>  the VAE: Q [128 x 512] (128 KB) + K [64 x 512] (64 KB) + V [64 x 256] (32 KB) = 224 KB, which is
-//                     why K / V are single-buffered. O [64 x 256] takes 128 fp32 registers per thread, so a CTA computes
-//                     one half of V / O and both halves recompute S (the score FLOPs double; they are 1/5 of a decoder
-//                     that is itself < 1 % of a 200-step generation). bf16 only: the VAE's parity mode keeps the
+//                     why K / V are single-buffered and refilled in line by thread 0 (with a producer warp, 3 warps on
+//                     one sub-partition would leave 168 registers per thread, and the kernel needs 197). O [64 x 256]
+//                     takes 128 fp32 registers per thread, so a CTA computes one half of V / O and both halves
+//                     recompute S (the score FLOPs double; they are 1/5 of a decoder that is itself < 1 % of a
+//                     200-step generation). bf16 only: the VAE's parity mode keeps the
 //                     GEMM -> softmax -> GEMM formulation.
 // The key mask, the ragged last key tile, rows past Lq and the lo half of the output are features of the head-64 entry;
 // the VAE entry has none of them (no mask, L a multiple of 128, bf16 output).
@@ -28,7 +35,16 @@ constexpr int FA_BM = 128;                // queries per CTA
 constexpr int FA_BN = 64;                 // keys per tile
 constexpr int FA_QCHUNK = FA_BM * 128;    // one [128][64] bf16 swizzled chunk = 16 KB
 constexpr int FA_KCHUNK = FA_BN * 128;    // one [64][64] bf16 swizzled chunk = 8 KB
-constexpr int FA_THREADS = 256;
+constexpr int FA_CONSUMERS = 256;        // two warpgroups
+// + the producer warp when the K / V ring is more than one buffer deep
+constexpr int fa_threads(int nbuf) { return nbuf > 1 ? FA_CONSUMERS + 32 : FA_CONSUMERS; }
+// Exponentials of the head-64 bf16 entry that run on the FMA pipe (ex2_poly) instead of MUFU: every FA_POLY_EVERY-th
+// of each row, 0 = none. A 64-key tile costs as many MUFU clocks (4096 ex2 at 16 / clk / SM) as tensor clocks, but the
+// kernel is bound by instruction issue, not by MUFU: ex2_poly is 10 instructions where ex2.approx is one. At B = 16,
+// 5 heads, 4096 x 4096 (H100 80GB HBM3, 700 W) every 4th exponential on ex2_poly made the kernel 894 us against 793 us
+// with none; before the scale was folded into the exponent's FMA, every 4th / 3rd / 2nd took it from 957 us to 1068 /
+// 1090 / 1178 us.
+constexpr int FA_POLY_EVERY = 0;
 
 struct AttnParams {
   int Lq, Lk;
@@ -51,7 +67,7 @@ struct FlashCfg {
 };
 
 template <int D, int DV, int NSPLIT, int NBUF>
-__global__ void __launch_bounds__(FA_THREADS, (D == 64 && NSPLIT == 1) ? 2 : 1)
+__global__ void __launch_bounds__(fa_threads(NBUF), (D == 64 && NSPLIT == 1) ? 2 : 1)
 flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant__ CUtensorMap kmap,
                        const __grid_constant__ CUtensorMap vmap, const __grid_constant__ AttnParams p) {
   using Cfg = FlashCfg<D, DV, NSPLIT, NBUF>;
@@ -100,6 +116,7 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_co
                     p.v_col0 + s * p.v_lo_off + vo_col + 64 * c, t * FA_BN, b);
   };
 
+  constexpr bool PRODUCER = NBUF > 1;
   if (tid == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();   // SWIZZLE_128B tiles need a 1024-byte aligned base
     tma_prefetch_desc(&qmap);
@@ -113,15 +130,36 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_co
       mbar_init(&empty_v[i], 2);
     }
     fence_mbar_init();
+  }
+  __syncthreads();
+  auto load_q = [&] {
     mbar_arrive_expect_tx(bar_q, Cfg::Q_BYTES);
 #pragma unroll
     for (int s = 0; s < NSPLIT; ++s)
 #pragma unroll
       for (int c = 0; c < DC; ++c)
         tma_load_3d(sQ + (s * DC + c) * FA_QCHUNK, &qmap, bar_q, p.q_col0 + s * p.q_lo_off + qk_col + 64 * c, q0, b);
-    for (int t = 0; t < NBUF && t < n_tiles; ++t) { load_k(t); load_v(t); }
+  };
+  if (!PRODUCER && tid == 0) {
+    load_q();
+    load_k(0);
+    load_v(0);
   }
-  __syncthreads();
+
+  if (PRODUCER && tid >= FA_CONSUMERS) {   // ---- the producer warp: Q once, then the K / V ring
+    if (tid == FA_CONSUMERS) {
+      load_q();
+      for (int t = 0; t < n_tiles; ++t) {
+        // buffer t % NBUF last held tile t - NBUF; both warpgroups release its K after S and its V after PV
+        const uint32_t ph = ((t / NBUF) & 1) ^ 1;
+        if (t >= NBUF) mbar_wait(&empty_k[t % NBUF], ph);
+        load_k(t);
+        if (t >= NBUF) mbar_wait(&empty_v[t % NBUF], ph);
+        load_v(t);
+      }
+    }
+    return;
+  }
 
   constexpr int NT = (NSPLIT == 1) ? 1 : 3;   // split products: hi*hi, lo*hi, hi*lo
   const int qsel[3] = {0, 1, 0}, ksel[3] = {0, 0, 1};
@@ -144,15 +182,6 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_co
   for (int t = 0; t < n_tiles; ++t) {
     const int buf = t % NBUF;
     const uint32_t ph = (t / NBUF) & 1;
-    // refill the buffers of tile t - 1 (released by both warpgroups at the end of that tile) with tile t - 1 + NBUF
-    if (NBUF > 1 && tid == 0 && t >= 1 && t - 1 + NBUF < n_tiles) {
-      const int pb = (t - 1) % NBUF;
-      const uint32_t pph = ((t - 1) / NBUF) & 1;
-      mbar_wait(&empty_k[pb], pph);
-      load_k(t - 1 + NBUF);
-      mbar_wait(&empty_v[pb], pph);
-      load_v(t - 1 + NBUF);
-    }
     // ---- S = Q K^T over the 64 keys of tile t
     float s[32];
     mbar_wait(&full_k[buf], ph);
@@ -172,32 +201,39 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_co
     wgmma_wait<0>();
     fence_regs(s);
     if ((tid & 127) == 0) mbar_arrive(&empty_k[buf]);
-    // a single buffer is refilled as soon as both warpgroups are done with it
-    if (NBUF == 1 && tid == 0 && t + 1 < n_tiles) {
+    // without a producer the single buffer is refilled as soon as both warpgroups are done with it
+    if (!PRODUCER && tid == 0 && t + 1 < n_tiles) {
       mbar_wait(&empty_k[buf], ph);
       load_k(t + 1);
     }
 
     // ---- online softmax (log2 domain); keys >= Lk score -inf. The mask test is compiled out of the VAE, which has no
     // masked keys: its per-element branches between S and the softmax made the VAE at B = 8, L = 4096 take 750 instead
-    // of 630 us (H100 80GB HBM3, 700 W power limit).
+    // of 630 us (H100 80GB HBM3, 700 W power limit). The test is one branch per tile, not one per score, and on full
+    // unmasked tiles the head-64 bf16 entry leaves S unscaled: softmax_step folds the scale into the FMA in front of
+    // each exponential. The parity mode and the VAE scale S first, as a separate rounding, so their arithmetic is
+    // unchanged.
     const int kv0 = t * FA_BN;
     const bool tail = D == 64 && ((kb != nullptr) || (kv0 + FA_BN > p.Lk));
+    const bool fold = D == 64 && NSPLIT == 1 && !tail;
+    if (tail) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < 8; ++j) {
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float bias = 0.f;
-        if (tail) {
+        for (int e = 0; e < 2; ++e) {
           const int kv = kv0 + 8 * j + 2 * t4 + e;
-          bias = kv < p.Lk ? (kb ? __ldg(kb + kv) * LOG2E : 0.f) : -INFINITY;
+          const float bias = kv < p.Lk ? (kb ? __ldg(kb + kv) * LOG2E : 0.f) : -INFINITY;
+          s[4 * j + e] = fmaf(s[4 * j + e], sc, bias);
+          s[4 * j + 2 + e] = fmaf(s[4 * j + 2 + e], sc, bias);
         }
-        s[4 * j + e] = fmaf(s[4 * j + e], sc, bias);
-        s[4 * j + 2 + e] = fmaf(s[4 * j + 2 + e], sc, bias);
       }
+    } else if (!fold) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = fmaf(s[i], sc, 0.f);
     }
     float corr[2];
-    softmax_step(s, m_run, l_run, corr);
+    // the parity mode keeps every exponential on ex2.approx (it is held to 1e-3 of fp32), and so does the VAE
+    softmax_step<(D == 64 && NSPLIT == 1) ? FA_POLY_EVERY : 0>(s, fold ? sc : 1.f, m_run, l_run, corr);
 #pragma unroll
     for (int n = 0; n < NV; ++n) rescale_rows(o[n], corr);
     uint32_t pa[NSPLIT][4][4];
@@ -224,7 +260,7 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_co
 #pragma unroll
     for (int n = 0; n < NV; ++n) fence_regs(o[n]);
     if ((tid & 127) == 0) mbar_arrive(&empty_v[buf]);
-    if (NBUF == 1 && tid == 0 && t + 1 < n_tiles) {
+    if (!PRODUCER && tid == 0 && t + 1 < n_tiles) {
       mbar_wait(&empty_v[buf], ph);
       load_v(t + 1);
     }
@@ -263,7 +299,7 @@ static int launch_flash(const void* q, long long ld_q, const void* k, long long 
   if (rc) return rc;
   dim3 grid((p.Lq + FA_BM - 1) / FA_BM, ny, batch);
   flash_attention_kernel<D, DV, NSPLIT, NBUF>
-      <<<grid, FA_THREADS, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(qm, km, vm, p);
+      <<<grid, fa_threads(NBUF), smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(qm, km, vm, p);
   return check_launch(what);
 }
 

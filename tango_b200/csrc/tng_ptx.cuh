@@ -230,6 +230,21 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// 2^x for x <= 0 on the FMA pipe instead of MUFU (which does 16 ex2 per clock per SM against 128 FMAs): x = n + f with
+// n = floor(x) (a round-down add of 1.5 * 2^23 leaves n in the low mantissa bits of t), 2^f on [0, 1] by a degree-4
+// minimax polynomial with p(0) = 1 in Horner form, then a multiply by 2^n built from t's bits. It agrees with
+// ex2.approx.ftz at the edges the softmax reaches: -inf -> +0, x < -126 -> +0 (2^n is +0 for n = -127, the clamp),
+// 0 -> exactly 1. Relative error <= 2^-18 over [-126, 0] (tests/test_attention_exp2_cpu.py states it in torch).
+__device__ __forceinline__ float ex2_poly(float x) {
+  x = fmaxf(x, -127.0f);
+  const float t = __fadd_rd(x, 12582912.0f);
+  const float f = x - (t - 12582912.0f);
+  float p = fmaf(0x1.b7ea5cp-7f, f, 0x1.abfe7ep-5f);
+  p = fmaf(p, f, 0x1.ee2374p-3f);
+  p = fmaf(p, f, 0x1.62d6d0p-1f);
+  p = fmaf(p, f, 1.0f);
+  return p * __int_as_float((__float_as_int(t) << 23) + 0x3f800000);
+}
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -328,11 +343,20 @@ __device__ __forceinline__ void store_bf16_split(__nv_bfloat16* p, float v, int 
 // of its warp's 16, s[4j + {0, 1}] of row r and s[4j + {2, 3}] of row r + 8. Index 0 / 1 of the per-row arrays below is
 // row r / r + 8; l_run is this lane's partial sum (the quad's lanes are combined by softmax_inv).
 //
-// One online-softmax step in the log2 domain: s holds the scaled scores (masked keys at -inf) and becomes the
-// unnormalised probabilities 2^(s - m); m_run / l_run are updated; corr receives the factor by which everything
-// accumulated over the previous tiles must be scaled. A row whose scores are all -inf so far keeps m_run = -inf and
-// gets probabilities 0 (instead of the NaN of -inf - -inf).
-__device__ __forceinline__ void softmax_step(float (&s)[32], float (&m_run)[2], float (&l_run)[2], float (&corr)[2]) {
+// One online-softmax step in the log2 domain: s * scl are the scaled scores (masked keys at -inf) and s becomes the
+// unnormalised probabilities 2^(s * scl - m), one FMA and one ex2 per score; m_run / l_run are updated; corr receives
+// the factor by which everything accumulated over the previous tiles must be scaled. scl > 0, so the row maximum of
+// s * scl is the maximum of s times scl; with scl = 1 the FMA is exactly s - m. A row whose scores are all -inf so far
+// keeps m_run = -inf and gets probabilities 0 (instead of the NaN of -inf - -inf).
+// POLY_EVERY > 0 moves every POLY_EVERY-th exponential of each row (a fixed set of registers) from MUFU to ex2_poly.
+template <int POLY_EVERY = 0>
+__device__ __forceinline__ void softmax_step(float (&s)[32], float scl, float (&m_run)[2], float (&l_run)[2],
+                                             float (&corr)[2]) {
+  auto ex2 = [](float x, int k) {
+    if constexpr (POLY_EVERY > 0)
+      if (k % POLY_EVERY == POLY_EVERY - 1) return ex2_poly(x);
+    return ex2_approx(x);
+  };
   float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -345,7 +369,7 @@ __device__ __forceinline__ void softmax_step(float (&s)[32], float (&m_run)[2], 
   float m_use[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const float m_new = fmaxf(m_run[h], quad_max(mx[h]));
+    const float m_new = fmaxf(m_run[h], quad_max(mx[h]) * scl);
     m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
     corr[h] = ex2_approx(m_run[h] - m_use[h]);   // 0 on the first tile (m_run = -inf)
     m_run[h] = m_new;
@@ -355,8 +379,8 @@ __device__ __forceinline__ void softmax_step(float (&s)[32], float (&m_run)[2], 
   for (int j = 0; j < 8; ++j) {
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      s[4 * j + e] = ex2_approx(s[4 * j + e] - m_use[0]);
-      s[4 * j + 2 + e] = ex2_approx(s[4 * j + 2 + e] - m_use[1]);
+      s[4 * j + e] = ex2(fmaf(s[4 * j + e], scl, -m_use[0]), 2 * j + e);
+      s[4 * j + 2 + e] = ex2(fmaf(s[4 * j + 2 + e], scl, -m_use[1]), 16 + 2 * j + e);
       l_run[0] += s[4 * j + e];
       l_run[1] += s[4 * j + 2 + e];
     }
