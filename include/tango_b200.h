@@ -222,6 +222,9 @@ int tng_transpose_bf16(const void* x, int64_t B, int64_t R, int64_t C, int64_t l
  * model_out: fp32 channels-last [(2)B, HW, C] (uncond half first when cfg); sample/noise/prev: fp32 NCHW
  * [B, C, HW] (the reference's latent layout); also writes next_in: the channels-last bf16 UNet input
  * [(2)B, HW, ld_in] for the next step (latents duplicated for the two CFG halves, hi/lo split optional).
+ * Returns TNG_EINVAL, before any CUDA call, unless: the required pointers are non-NULL (sample, coef, and prev or
+ * next_in); B, C, HW >= 1; ld_mo >= C when model_out is given; with next_in, split_off is 0 or >= C and
+ * ld_in >= C + split_off. tng_dpm_step and tng_latent_blend make the same checks.
  */
 int tng_sched_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
                    const float* noise, const float* coef, float* prev, void* next_in, int64_t ld_in,
@@ -244,7 +247,8 @@ int tng_sched_step(const float* model_out, int64_t ld_mo, int32_t cfg, float gui
  * converted outputs of this, the previous and the one-before step; m1 is needed for order >= 2, m2 for order 3)
  * and prev: fp32 NCHW [B, C, HW]; prev may alias sample. The caller rotates the history slots. Also writes
  * next_in: the channels-last bf16 UNet input [(2)B, HW, ld_in] (duplicated for the CFG halves, hi/lo split at
- * split_off when > 0).
+ * split_off when > 0). TNG_EINVAL as tng_sched_step (required: model_out, sample, coef, m0, and prev or next_in), and
+ * for an order outside 1-3 or a missing history slot.
  */
 int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
                  const float* coef, int32_t order, float* m0, const float* m1, const float* m2, float* prev,
@@ -263,7 +267,7 @@ int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guida
  * [B, C, HW]; sample is read only under a mask and may not alias x0 or noise. mask: fp32 [Bm, HW], entry b at
  * mask + b * mask_bstride (0 broadcasts one mask over the batch). Optionally also writes next_in: the channels-last
  * bf16 UNet input [(2)B, HW, ld_in] (duplicated for the CFG halves when cfg, hi/lo split at split_off when > 0), as
- * tng_sched_step packs it.
+ * tng_sched_step packs it. TNG_EINVAL as tng_sched_step (required: x0, coef, sample), and for mask_bstride < 0.
  */
 int tng_latent_blend(const float* x0, const float* noise, const float* mask, int64_t mask_bstride, const float* coef,
                      float* sample, void* next_in, int64_t ld_in, int32_t cfg, int32_t split_off, int64_t B, int64_t C,

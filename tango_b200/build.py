@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libtango_b200.so")
-SOURCES = ["capi.cu", "gemm_tc.cu", "attention.cu", "elementwise.cu", "dpm_solver.cu", "latent_blend.cu"]
+SOURCES = ["capi.cu", "gemm_tc.cu", "attention.cu", "elementwise.cu", "latent_step.cu"]
 HEADERS = ["tng_ptx.cuh", "tng_internal.h", os.path.join("..", "..", "include", "tango_b200.h")]
 
 NVCC_FLAGS = [

@@ -434,50 +434,6 @@ __global__ void __launch_bounds__(256) transpose_bf16_kernel(const __nv_bfloat16
   }
 }
 
-// ------------------------------------------------------------------------------------------------ CFG + scheduler
-__global__ void __launch_bounds__(256) sched_step_kernel(const float* mo, long long ld_mo, int cfg, float guidance,
-                                                          const float* sample, const float* noise, const float* coef,
-                                                          float* prev, __nv_bfloat16* next_in, long long ld_in,
-                                                          int split_off, long long B, int C, long long HW) {
-  const float c_x0_s = coef[0], c_x0_m = coef[1], c_prev_x0 = coef[2], c_prev_s = coef[3], c_noise = coef[4];
-  const float c_eps_s = coef[5], c_eps_m = coef[6], c_prev_eps = coef[7], clip = coef[8], c_x0_div = coef[9];
-  const long long total = B * HW * C;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % C);
-    const long long hw = (i / C) % HW;
-    const long long b = i / (C * HW);
-    const long long nchw = (b * C + c) * HW + hw;
-    const float s = sample[nchw];
-    float out = s;
-    if (mo) {
-      float v;
-      if (cfg) {
-        const float u = mo[(b * HW + hw) * ld_mo + c];
-        const float t = mo[((B + b) * HW + hw) * ld_mo + c];
-        v = __fadd_rn(u, __fmul_rn(guidance, __fsub_rn(t, u)));  // models.py:246, no fma contraction
-      } else {
-        v = mo[(b * HW + hw) * ld_mo + c];
-      }
-      // scheduling_ddpm.py:306-311 / scheduling_ddim.py:303-313 with host-computed fp32 coefficients; the
-      // multiplications and additions keep the reference's association order (no fma contraction).
-      float x0 = __fdiv_rn(__fadd_rn(__fmul_rn(c_x0_s, s), __fmul_rn(c_x0_m, v)), c_x0_div);
-      if (clip > 0.f) x0 = fminf(fmaxf(x0, -clip), clip);
-      out = __fadd_rn(__fmul_rn(c_prev_x0, x0), __fmul_rn(c_prev_s, s));
-      if (c_prev_eps != 0.f) {
-        const float eps = __fadd_rn(__fmul_rn(c_eps_s, s), __fmul_rn(c_eps_m, v));
-        out = __fadd_rn(out, __fmul_rn(c_prev_eps, eps));
-      }
-      if (noise && c_noise != 0.f) out = __fadd_rn(out, __fmul_rn(c_noise, noise[nchw]));
-    }
-    if (prev) prev[nchw] = out;
-    if (next_in) {
-      store_bf16_split(next_in + (b * HW + hw) * ld_in + c, out, split_off);
-      if (cfg) store_bf16_split(next_in + ((B + b) * HW + hw) * ld_in + c, out, split_off);
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ time embedding
 __global__ void timestep_embedding_kernel(const float* t, long long n, int dim, int flip, float freq_shift, float* out) {
   const int half = dim / 2;
@@ -620,14 +576,6 @@ static inline unsigned ln_grid(long long rows, int wpb) {
   const long long cap = 4LL * num_sms();
   if (g > cap) g = cap;
   return static_cast<unsigned>(g < 1 ? 1 : g);
-}
-
-static inline int grid_for(long long total, int block = 256) {
-  long long g = (total + block - 1) / block;
-  const long long cap = static_cast<long long>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
 }
 
 }  // namespace tng
@@ -776,16 +724,6 @@ extern "C" int tng_transpose_bf16(const void* x, int64_t B, int64_t R, int64_t C
   transpose_bf16_kernel<<<grid, 256, 0, ST(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(x), (int)R, (int)C, ld_x,
                                                        reinterpret_cast<__nv_bfloat16*>(y), ld_y);
   return check_launch("transpose");
-}
-
-extern "C" int tng_sched_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
-                              const float* noise, const float* coef, float* prev, void* next_in, int64_t ld_in,
-                              int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream) {
-  if (!sample || !coef || (!prev && !next_in)) return set_error(TNG_EINVAL, "sched_step: null argument");
-  sched_step_kernel<<<grid_for(B * C * HW), 256, 0, ST(stream)>>>(model_out, ld_mo, cfg, guidance, sample, noise, coef, prev,
-                                                                  reinterpret_cast<__nv_bfloat16*>(next_in), ld_in,
-                                                                  split_off, B, (int)C, HW);
-  return check_launch("sched_step");
 }
 
 extern "C" int tng_timestep_embedding(const float* t, int64_t n, int32_t dim, int32_t flip_sin_to_cos, float freq_shift,

@@ -12,6 +12,14 @@ namespace tng {
 int set_error(int code, const char* fmt, ...);
 int num_sms();
 void count_launch();
+// Grid of an elementwise kernel over `total` items: one item per thread up to 16 CTAs per SM, then the threads stride
+inline int grid_for(long long total, int block = 256) {
+  long long g = (total + block - 1) / block;
+  const long long cap = static_cast<long long>(num_sms()) * 16;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return static_cast<int>(g);
+}
 // Encode a bf16 tiled tensor map with SWIZZLE_128B and zero OOB fill (driver entry point resolved at run time so
 // the library loads on machines without libcuda).
 int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,

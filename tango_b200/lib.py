@@ -385,11 +385,16 @@ def transpose_bf16(x, B, R, Cc, y):
           y.data_ptr(), y.stride(0), stream_ptr())
 
 
+def _next_in_bytes(next_in, n, cfg, split_off):
+    """Bytes a latent update writes to the next UNet input: n bf16 values, twice under CFG, hi and lo when split."""
+    return 0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2)
+
+
 def sched_step(model_out, cfg, guidance, sample, noise, coef, prev, next_in, *, B, Cc, HW, split_off=0):
     require_cuda(model_out, sample, noise, coef, prev, next_in)
     n = B * Cc * HW
     nbytes = n * 4 * ((2 if cfg else 1) * (model_out is not None) + 1 + (noise is not None) + (prev is not None)) \
-        + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
+        + _next_in_bytes(next_in, n, cfg, split_off)
     _call("sched_step", nbytes, load().tng_sched_step, ptr(model_out), 0 if model_out is None else model_out.stride(0),
           int(cfg), guidance, sample.data_ptr(), ptr(noise), coef.data_ptr(), ptr(prev), ptr(next_in),
           0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
@@ -401,7 +406,7 @@ def dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, ne
     require_cuda(model_out, sample, coef, m0, m1, m2, prev, next_in)
     n = B * Cc * HW
     nbytes = n * 4 * ((2 if cfg else 1) + 1 + 1 + (order - 1) + (prev is not None)) \
-        + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
+        + _next_in_bytes(next_in, n, cfg, split_off)
     _call("dpm_step", nbytes, load().tng_dpm_step, model_out.data_ptr(), model_out.stride(0), int(cfg), guidance,
           sample.data_ptr(), coef.data_ptr(), order, m0.data_ptr(), ptr(m1), ptr(m2), ptr(prev), ptr(next_in),
           0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
@@ -419,7 +424,7 @@ def latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW, cfg=
         mstride = 0 if mask.numel() == HW else HW
     n = B * Cc * HW
     nbytes = n * 4 * (1 + (noise is not None) + (mask is not None) + 1) + (0 if mask is None else mask.numel() * 4) \
-        + (0 if next_in is None else n * (2 if cfg else 1) * (4 if split_off else 2))
+        + _next_in_bytes(next_in, n, cfg, split_off)
     _call("latent_blend", nbytes, load().tng_latent_blend, x0.data_ptr(), ptr(noise), ptr(mask), mstride,
           coef.data_ptr(), sample.data_ptr(), ptr(next_in), 0 if next_in is None else next_in.stride(0), int(cfg),
           split_off, B, Cc, HW, stream_ptr())

@@ -8,7 +8,7 @@ scheduling_ddim.py:132-359; call sites models.py:224-249, tango.py:36): `set_tim
 (scheduling_dpmsolver_multistep.py:57-535) is the opt-in few-step sampler; its update runs in tng_dpm_step (below).
 
 All per-step scalars are computed on the host with the reference's own fp32 torch ops (same association order),
-packed into a [num_steps, 10] coefficient table and shipped to the device once per `set_timesteps`; the kernel
+packed into a [num_steps, 10] coefficient table and shipped to the device once per timestep grid; the kernel
 (tng_sched_step) then evaluates  x0 = (c0*s + c1*v)/c9, prev = c2*x0 + c3*s + c7*(c5*s + c6*v) + c4*noise  with
 un-fused multiplies/adds, which reproduces the reference CPU arithmetic bit for bit and removes the two host syncs
 per step of the reference (SURVEY.md §1).
@@ -62,9 +62,9 @@ class _SchedulerBase:
         self.init_noise_sigma = 1.0
         self.num_inference_steps: Optional[int] = None
         self.timesteps = torch.from_numpy(np.arange(0, cfg["num_train_timesteps"])[::-1].copy().astype(np.int64))
-        self._coef_host: Optional[torch.Tensor] = None   # [num_steps, NCOEF] fp32 (CPU)
-        self._coef_dev: Optional[torch.Tensor] = None
+        self._t_list: Optional[list] = None
         self._t_index: dict = {}
+        self._tables: dict = {}   # (kind, grid, t_start) -> (host table, DPM loop orders or None, {device: copy})
 
     @classmethod
     def from_pretrained(cls, name: str = "stabilityai/stable-diffusion-2-1", subfolder: str = "scheduler", **overrides):
@@ -114,21 +114,34 @@ class _SchedulerBase:
 
     def _finish_set_timesteps(self, device):
         self._t_list = [int(t) for t in self.timesteps.tolist()]
-        key = tuple(self._t_list)
-        cache = self.__dict__.setdefault("_table_cache", {})
-        if key not in cache:   # ~40 tiny fp32 torch ops per step: computed once per grid, reused by later calls
-            cache[key] = torch.stack(self._table_rows()).contiguous()
-        self._coef_host = cache[key]
         self._t_index = {t: i for i, t in enumerate(self._t_list)}
-        self._coef_dev = None
         if device is not None:
             self.timesteps = self.timesteps.to(device)
-            if torch.device(device).type == "cuda":
-                self._coef_dev = self._coef_host.to(device)
+        self.coefficient_table(device)
 
-    def _table_rows(self) -> list:
-        """Row i of the coefficient table belongs to timesteps[i]."""
-        return [self._coefficients(t) for t in self._t_list]
+    def _table(self, kind: str, device=None, t_start: int = 0):
+        """(table, loop orders) of the current grid for a loop entered at timesteps[t_start]; row i belongs to
+        timesteps[i]. kind "coef" is the update's coefficient table, "blend" the add_noise rows. Each (kind, grid,
+        t_start) is computed once (~40 tiny fp32 torch ops per row) and copied to each device once; `device` None
+        gives the host table."""
+        if self._t_list is None:
+            self._finish_set_timesteps(None)
+        key = (kind, tuple(self._t_list), t_start)
+        if key not in self._tables:
+            rows, orders = self._table_rows(kind, t_start)
+            self._tables[key] = (torch.stack(rows).contiguous(), orders, {})
+        host, orders, dev = self._tables[key]
+        if device is None:
+            return host, orders
+        d = str(torch.device(device))
+        if d not in dev:
+            dev[d] = host.to(device)
+        return dev[d], orders
+
+    def _table_rows(self, kind: str, t_start: int):
+        """The rows of table `kind` and the loop orders they belong to (None: they do not depend on the order)."""
+        row = self._blend_row if kind == "blend" else self._coefficients
+        return [row(t) for t in self._t_list], None
 
     def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
         """Coefficient table of a loop that runs timesteps[t_start:] (row i belongs to timesteps[i]); only the
@@ -156,19 +169,7 @@ class _SchedulerBase:
     def blend_table(self, device=None) -> torch.Tensor:
         """[num_steps, 2] fp32 add_noise coefficients of the current grid (row i belongs to timesteps[i]): the
         coefficient rows of tng_latent_blend."""
-        if self._coef_host is None:
-            self._finish_set_timesteps(None)
-        cache = self.__dict__.setdefault("_blend_cache", {})
-        key = tuple(self._t_list)
-        if key not in cache:
-            cache[key] = torch.stack([self._blend_row(t) for t in self._t_list]).contiguous()
-        tab = cache[key]
-        if device is None:
-            return tab
-        dkey = (key, str(torch.device(device)))
-        if dkey not in cache:
-            cache[dkey] = tab.to(device)
-        return cache[dkey]
+        return self._table("blend", device)[0]
 
     def add_noise(self, original_samples: torch.Tensor, noise: torch.Tensor, timesteps) -> torch.Tensor:
         """scheduling_ddpm.py:351-372 (DDIM and DPM-Solver share it) for fp32 CUDA tensors of shape (B, C, ...):
@@ -206,30 +207,18 @@ class _SchedulerBase:
 
     def coefficient_table(self, device=None) -> torch.Tensor:
         """[num_steps, 10] fp32 table (row i belongs to timesteps[i])."""
-        if self._coef_host is None:
-            self._finish_set_timesteps(None)
-        if device is None:
-            return self._coef_host
-        if self._coef_dev is None or self._coef_dev.device != torch.device(device):
-            self._coef_dev = self._coef_host.to(device)
-        return self._coef_dev
-
-    def _row(self, timestep) -> int:
-        t = int(timestep)
-        if self._coef_host is None or t not in self._t_index:
-            # arbitrary timestep outside the current grid (the reference allows it): one-row table
-            self._coef_host = self._coefficients(t)[None].contiguous()
-            self._t_index = {t: 0}
-            self._coef_dev = None
-        return self._t_index[t]
+        return self._table("coef", device)[0]
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, generator=None,
              variance_noise: Optional[torch.Tensor] = None, return_dict: bool = True, **_unused):
         """x_t -> x_{t-1} for NCHW fp32 CUDA tensors (reference layout). Noise comes from the torch RNG exactly as
         in the reference (randn of model_output's shape when t > 0) unless `variance_noise` is given."""
         L.require_cuda(model_output)   # no CPU fallback
-        i = self._row(timestep)
-        coef = self.coefficient_table(sample.device)[i]
+        i = self._t_index.get(int(timestep))
+        if i is None:   # a timestep outside the grid (the reference allows it) gets a row of its own
+            coef = self._coefficients(int(timestep)).to(sample.device)
+        else:
+            coef = self.coefficient_table(sample.device)[i]
         B, Cc, H, W = sample.shape
         noise = None
         if self._needs_noise(int(timestep)):
@@ -445,31 +434,20 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
 
     def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
         """The coefficient table of a loop entered at timesteps[t_start] (an edit): its rows come from
-        `_coefficients_at` with the mid-grid orders, cached per (grid, t_start). t_start = 0 is the `set_timesteps`
-        table itself."""
-        if t_start == 0:
-            self._loop_orders = self._orders
-            return self.coefficient_table(device)
-        cache = self.__dict__.setdefault("_mid_cache", {})
-        key = (tuple(self._t_list), t_start)
-        if key not in cache:
-            orders = self._loop_orders_from(len(self._t_list), t_start)
-            rows = [self._coef_host[i] for i in range(t_start)] + \
-                [self._coefficients_at(i, orders[i]) for i in range(t_start, len(self._t_list))]
-            cache[key] = (orders, torch.stack(rows).contiguous(), {})
-        orders, host, dev = cache[key]
-        self._loop_orders = orders
-        d = str(torch.device(device))
-        if d not in dev:
-            dev[d] = host.to(device)
-        return dev[d]
+        `_coefficients_at` with the mid-grid orders, which `_loop_step` then follows. t_start = 0 is the
+        `set_timesteps` table itself."""
+        tab, self._loop_orders = self._table("coef", device, t_start)
+        return tab
 
     def order_at(self, i: int) -> int:
         """Order of step i in a loop started by `set_timesteps`."""
         return self._orders[i]
 
-    def _table_rows(self) -> list:
-        return [self._coefficients_at(i, self._orders[i]) for i in range(len(self._t_list))]
+    def _table_rows(self, kind: str, t_start: int):
+        if kind != "coef":
+            return super()._table_rows(kind, t_start)
+        orders = self._loop_orders_from(len(self._t_list), t_start)
+        return [self._coefficients_at(i, o) for i, o in enumerate(orders)], orders
 
     def _coefficients_at(self, i: int, order: int, timestep: Optional[int] = None) -> torch.Tensor:
         """The fp32 scalars of step index i at `order` (:243-281, :305-427, same torch ops in the same order).

@@ -88,9 +88,10 @@ def spec_conv_gemm(views, groups, weight, W, H, NB, *, bias=None, rowvec=None, r
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# The other entry points of include/tango_b200.h, same purpose: torch-CPU statements of the contracts, used by
-# tests/test_orchestration_spec.py to run the package's host orchestration (weight packing, buffer plumbing, operator
-# sequencing of unet.py / t5.py) without a GPU. Every function mirrors the signature of its tango_b200.lib wrapper.
+# The other entry points of include/tango_b200.h, same purpose: torch-CPU statements of the contracts, installed by
+# `install_spec_backend` to run the package's host orchestration (weight packing, buffer plumbing, operator sequencing
+# of unet.py / t5.py, the sampling and editing loops) without a GPU. Every function mirrors the signature of its
+# tango_b200.lib wrapper.
 def _store_bf16(y, z, split_off):
     hi = z.to(torch.bfloat16)
     n = z.shape[1]
@@ -236,20 +237,35 @@ def spec_tanh_to_i16(x, n, ld_x, wave_f32, wave_i16):
         wave_i16.reshape(-1)[:n] = (t * 32768.0).to(torch.int32).to(torch.int16)
 
 
+# The latent updates (tng_sched_step, tng_dpm_step, tng_latent_blend): one op per kernel op, same association.
+# model_out: channels-last rows [(2)B*HW, >=Cc] fp32; sample / noise / prev / history: NCHW fp32; next_in: channels-last
+# bf16 rows [(2)B*HW, ld_in].
+def _guided_output(model_out, cfg, guidance, *, B, Cc, HW):
+    """The model output as [B, Cc, HW]: u + guidance * (t - u) under CFG (uncond rows first)."""
+    mo = model_out[:, :Cc].float()
+    if cfg:
+        u, t = mo[:B * HW].reshape(B, HW, Cc), mo[B * HW:2 * B * HW].reshape(B, HW, Cc)
+        v = u + guidance * (t - u)
+    else:
+        v = mo[:B * HW].reshape(B, HW, Cc)
+    return v.transpose(1, 2)
+
+
+def _pack_next_in(next_in, x, cfg, split_off, *, B, Cc, HW):
+    """The new latent x [B, Cc, HW] as the next UNet input: once per CFG half, hi/lo split at split_off."""
+    if next_in is not None:
+        rows = x.transpose(1, 2).reshape(B * HW, Cc)
+        for r in range(2 if cfg else 1):
+            _store_bf16(next_in[r * B * HW:(r + 1) * B * HW], rows, split_off)
+
+
 def spec_sched_step(model_out, cfg, guidance, sample, noise, coef, prev, next_in, *, B, Cc, HW, split_off=0):
-    """CFG combine + scheduler update (coefficient row `coef`, see schedulers.py) + packing of the next UNet input.
-    model_out: channels-last rows [(2)B*HW, >=Cc] fp32; sample / noise / prev: NCHW fp32; next_in: channels-last bf16."""
+    """CFG combine + scheduler update (coefficient row `coef`, see schedulers.py) + packing of the next UNet input."""
     c = [coef.reshape(-1)[i] for i in range(10)]
     s = sample.reshape(B, Cc, HW).float()
     out = s
     if model_out is not None:
-        mo = model_out[:, :Cc].float()
-        if cfg:
-            u, t = mo[:B * HW].reshape(B, HW, Cc), mo[B * HW:2 * B * HW].reshape(B, HW, Cc)
-            v = u + guidance * (t - u)
-        else:
-            v = mo[:B * HW].reshape(B, HW, Cc)
-        v = v.transpose(1, 2)
+        v = _guided_output(model_out, cfg, guidance, B=B, Cc=Cc, HW=HW)
         x0 = (c[0] * s + c[1] * v) / c[9]
         if float(c[8]) > 0:
             x0 = x0.clamp(-float(c[8]), float(c[8]))
@@ -260,11 +276,40 @@ def spec_sched_step(model_out, cfg, guidance, sample, noise, coef, prev, next_in
             out = out + c[4] * noise.reshape(B, Cc, HW)
     if prev is not None:
         prev.reshape(B, Cc, HW).copy_(out)
-    if next_in is not None:
-        rows = out.transpose(1, 2).reshape(B * HW, Cc)
-        reps = 2 if cfg else 1
-        for r in range(reps):
-            _store_bf16(next_in[r * B * HW:(r + 1) * B * HW], rows, split_off)
+    _pack_next_in(next_in, out, cfg, split_off, B=B, Cc=Cc, HW=HW)
+
+
+def spec_dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, next_in, *, B, Cc, HW, split_off=0):
+    """CFG combine + DPM-Solver(++) update of `order` from the history slots m0 (written) / m1 / m2 + packing."""
+    c = [coef.reshape(-1)[i] for i in range(11)]
+    s = sample.reshape(B, Cc, HW).float()
+    v = _guided_output(model_out, cfg, guidance, B=B, Cc=Cc, HW=HW)
+    x0 = (c[0] * s + c[1] * v) / c[2]
+    m0.reshape(B, Cc, HW).copy_(x0)
+    x = c[3] * s - c[4] * x0
+    if order == 2:
+        x = x + c[5] * (c[7] * (x0 - m1.reshape(B, Cc, HW)))
+    elif order == 3:
+        p1, p2 = m1.reshape(B, Cc, HW), m2.reshape(B, Cc, HW)
+        d1_0, d1_1 = c[7] * (x0 - p1), c[8] * (p1 - p2)
+        dd = d1_0 - d1_1
+        x = (x + c[5] * (d1_0 + c[9] * dd)) - c[6] * (c[10] * dd)
+    if prev is not None:
+        prev.reshape(B, Cc, HW).copy_(x)
+    _pack_next_in(next_in, x, cfg, split_off, B=B, Cc=Cc, HW=HW)
+
+
+def spec_latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW, cfg=False, split_off=0):
+    """add_noise(x0, noise) (mask None) or add_noise(x0, noise) * m + sample * (1 - m), written to sample + packing."""
+    c = coef.reshape(-1)
+    p = c[0] * x0.reshape(B, Cc, HW).float()
+    if noise is not None:
+        p = p + c[1] * noise.reshape(B, Cc, HW).float()
+    if mask is not None:
+        m = mask.reshape(-1, 1, HW)
+        p = (p * m) + (sample.reshape(B, Cc, HW) * (1 - m))
+    sample.reshape(B, Cc, HW).copy_(p)
+    _pack_next_in(next_in, p, cfg, split_off, B=B, Cc=Cc, HW=HW)
 
 
 def spec_stft_frames(y, pad, hi, lo):
@@ -296,6 +341,20 @@ def spec_log_clamp(x, y, floor=1e-5):
 
 SPEC = {"attention_wide": spec_attention_wide, "stft_frames": spec_stft_frames, "stft_magnitude": spec_stft_magnitude, "log_clamp": spec_log_clamp,
         "softmax_rows": spec_softmax_rows, "transpose_bf16": spec_transpose_bf16, "convt_gather": spec_convt_gather,
-        "tanh_to_i16": spec_tanh_to_i16, "sched_step": spec_sched_step, "conv_gemm": spec_conv_gemm, "groupnorm": spec_groupnorm, "groupnorm_stats": spec_groupnorm_stats, "layernorm": spec_layernorm, "rmsnorm": spec_rmsnorm,
+        "tanh_to_i16": spec_tanh_to_i16, "sched_step": spec_sched_step, "dpm_step": spec_dpm_step,
+        "latent_blend": spec_latent_blend, "conv_gemm": spec_conv_gemm, "groupnorm": spec_groupnorm, "groupnorm_stats": spec_groupnorm_stats, "layernorm": spec_layernorm, "rmsnorm": spec_rmsnorm,
         "gather_rows": spec_gather_rows, "cast_act": spec_cast_act, "attention": spec_attention,
         "rel_attention": spec_rel_attention, "timestep_embedding": spec_timestep_embedding, "linear_f32": spec_linear_f32}
+
+
+def install_spec_backend(monkeypatch):
+    """Run the package's host code on CPU tensors: every kernel wrapper of tango_b200.lib becomes its statement in
+    SPEC, and the device checks, the library load and the launch counter become no-ops (under pytest's monkeypatch
+    only, so nothing here is a CPU fallback of the product)."""
+    from tango_b200 import lib as L
+    for name, fn in SPEC.items():
+        monkeypatch.setattr(L, name, fn)
+    monkeypatch.setattr(L, "require_cuda_device", lambda device: None)
+    monkeypatch.setattr(L, "require_cuda", lambda *ts: None)
+    monkeypatch.setattr(L, "load", lambda *a, **k: None)
+    monkeypatch.setattr(L, "launch_count", lambda: 0)

@@ -84,3 +84,39 @@ def test_linear_f32_rejects_activations_other_than_none_and_silu():
         rc = lib.tng_linear_f32(ctypes.addressof(x), 2, 8, ctypes.addressof(w), None, 4, pre, post, ctypes.addressof(y),
                                 None)
         assert rc == -1 and b"linear_f32" in lib.tng_last_error(), (pre, post)
+
+
+def test_latent_updates_reject_bad_arguments_before_any_launch():
+    """tng_sched_step, tng_dpm_step and tng_latent_blend share their checks: required pointers, B, C and HW >= 1,
+    ld_mo >= C, split_off 0 or >= C and ld_in >= C + split_off, plus each entry point's own. Every failure is TNG_EINVAL
+    naming the entry point, returned before any CUDA call, so host buffers and no device suffice."""
+    lib = L.load()
+    buf = ctypes.create_string_buffer(1 << 16)
+    p = ctypes.addressof(buf)
+    C = 4
+    common = dict(coef=p, next_in=p, ld_in=2 * C, split_off=C, cfg=1, B=2, C=C, HW=8, stream=None)
+    calls = {
+        "sched_step": (lib.tng_sched_step, "model_out ld_mo cfg guidance sample noise coef prev next_in ld_in "
+                       "split_off B C HW stream", dict(model_out=p, ld_mo=C, guidance=3.0, sample=p, noise=p, prev=p),
+                       ["sample", "coef"]),
+        "dpm_step": (lib.tng_dpm_step, "model_out ld_mo cfg guidance sample coef order m0 m1 m2 prev next_in ld_in "
+                     "split_off B C HW stream", dict(model_out=p, ld_mo=C, guidance=3.0, sample=p, order=3, m0=p, m1=p,
+                                                     m2=p, prev=p), ["model_out", "sample", "coef", "m0"]),
+        "latent_blend": (lib.tng_latent_blend, "x0 noise mask mask_bstride coef sample next_in ld_in cfg split_off B C "
+                         "HW stream", dict(x0=p, noise=p, mask=p, mask_bstride=8, sample=p), ["x0", "coef", "sample"]),
+    }
+    for name, (fn, argnames, own, required) in calls.items():
+        good = dict(common, **own)
+        bad = [{k: None} for k in required]
+        bad += [dict(B=0), dict(C=0), dict(HW=0), dict(B=-1), dict(split_off=1), dict(split_off=C - 1),
+                dict(split_off=-C), dict(ld_in=2 * C - 1), dict(split_off=0, ld_in=C - 1)]
+        if "ld_mo" in good:
+            bad += [dict(ld_mo=C - 1), dict(ld_mo=0), dict(prev=None, next_in=None)]
+        if name == "dpm_step":
+            bad += [dict(order=0), dict(order=4), dict(m1=None), dict(order=2, m1=None), dict(m2=None)]
+        if name == "latent_blend":
+            bad.append(dict(mask_bstride=-1))
+        for change in bad:
+            args = {**good, **change}
+            rc = fn(*[args[a] for a in argnames.split()])
+            assert rc == -1 and name.encode() in lib.tng_last_error(), (name, change, rc, lib.tng_last_error())

@@ -1,7 +1,7 @@
 """CPU: the multistep DPM-Solver(++) scheduler. The oracle is pinned to the fork's known answers and to
 tests/golden/dpm_solver.npz; the product's coefficient tables and its inference loop are driven through a torch
-statement of what tng_dpm_step computes (defined here) and must reproduce the reference bit for bit. Nothing here is a
-CPU fallback of the product: the substitution exists only under pytest's monkeypatch."""
+statement of what tng_dpm_step computes (cabi_spec.spec_dpm_step) and must reproduce the reference bit for bit. Nothing
+here is a CPU fallback of the product: the substitution exists only under pytest's monkeypatch."""
 import json
 import os
 
@@ -22,44 +22,9 @@ FORK_TEST = dict(num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, bet
                  lower_order_final=False, solver_order=2)
 
 
-def spec_dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, next_in, *, B, Cc, HW, split_off=0):
-    """tng_dpm_step (include/tango_b200.h) in torch fp32: one op per kernel op, same association."""
-    c = [coef.reshape(-1)[i] for i in range(11)]
-    s = sample.reshape(B, Cc, HW).float()
-    mo = model_out[:, :Cc].float()
-    if cfg:
-        u, t = mo[:B * HW].reshape(B, HW, Cc), mo[B * HW:2 * B * HW].reshape(B, HW, Cc)
-        v = u + guidance * (t - u)
-    else:
-        v = mo[:B * HW].reshape(B, HW, Cc)
-    v = v.transpose(1, 2)
-    x0 = (c[0] * s + c[1] * v) / c[2]
-    m0.reshape(B, Cc, HW).copy_(x0)
-    x = c[3] * s - c[4] * x0
-    if order == 2:
-        x = x + c[5] * (c[7] * (x0 - m1.reshape(B, Cc, HW)))
-    elif order == 3:
-        p1, p2 = m1.reshape(B, Cc, HW), m2.reshape(B, Cc, HW)
-        d1_0, d1_1 = c[7] * (x0 - p1), c[8] * (p1 - p2)
-        dd = d1_0 - d1_1
-        x = (x + c[5] * (d1_0 + c[9] * dd)) - c[6] * (c[10] * dd)
-    if prev is not None:
-        prev.reshape(B, Cc, HW).copy_(x)
-    if next_in is not None:
-        rows = x.transpose(1, 2).reshape(B * HW, Cc)
-        for r in range(2 if cfg else 1):
-            cabi_spec._store_bf16(next_in[r * B * HW:(r + 1) * B * HW], rows, split_off)
-
-
 @pytest.fixture
 def spec_backend(monkeypatch):
-    for name, fn in cabi_spec.SPEC.items():
-        monkeypatch.setattr(L, name, fn)
-    monkeypatch.setattr(L, "dpm_step", spec_dpm_step)
-    monkeypatch.setattr(L, "require_cuda_device", lambda device: None)
-    monkeypatch.setattr(L, "require_cuda", lambda *ts: None)
-    monkeypatch.setattr(L, "load", lambda *a, **k: None)
-    monkeypatch.setattr(L, "launch_count", lambda: 0)
+    cabi_spec.install_spec_backend(monkeypatch)
 
     class _NoEvent:
         def __init__(self, *a, **k):

@@ -1,8 +1,8 @@
 """CPU: text-guided editing and inpainting. The scheduler arithmetic (strength -> t_start, add_noise, blend rows, the
 orders of a DPM-Solver loop entered mid-grid) is held bit for bit to the fork's values in tests/golden/edit.npz
-(oracle/make_golden_edit.py); the edit and inpaint loops run through cabi_spec.SPEC plus `spec_latent_blend`, a torch
-statement of tng_latent_blend defined here. Nothing here is a CPU fallback of the product: the substitution exists only
-under pytest's monkeypatch."""
+(oracle/make_golden_edit.py); the edit and inpaint loops run through cabi_spec.SPEC, whose `spec_latent_blend` is a
+torch statement of tng_latent_blend. Nothing here is a CPU fallback of the product: the substitution exists only under
+pytest's monkeypatch."""
 import json
 import os
 
@@ -16,38 +16,14 @@ from tango_b200 import lib as L
 from tango_b200 import synth
 from tango_b200.pipeline import AudioDiffusion, Tango, ratio_mask
 from tango_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
-from test_dpm_solver_cpu import spec_dpm_step
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 CPU = torch.device("cpu")
 
 
-def spec_latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW, cfg=False, split_off=0):
-    """tng_latent_blend (include/tango_b200.h) in torch fp32: one op per kernel op, same association."""
-    c = coef.reshape(-1)
-    p = c[0] * x0.reshape(B, Cc, HW).float()
-    if noise is not None:
-        p = p + c[1] * noise.reshape(B, Cc, HW).float()
-    if mask is not None:
-        m = mask.reshape(-1, 1, HW)
-        p = (p * m) + (sample.reshape(B, Cc, HW) * (1 - m))
-    sample.reshape(B, Cc, HW).copy_(p)
-    if next_in is not None:
-        rows = p.transpose(1, 2).reshape(B * HW, Cc)
-        for r in range(2 if cfg else 1):
-            cabi_spec._store_bf16(next_in[r * B * HW:(r + 1) * B * HW], rows, split_off)
-
-
 @pytest.fixture
 def spec_backend(monkeypatch):
-    for name, fn in cabi_spec.SPEC.items():
-        monkeypatch.setattr(L, name, fn)
-    monkeypatch.setattr(L, "dpm_step", spec_dpm_step)
-    monkeypatch.setattr(L, "latent_blend", spec_latent_blend)
-    monkeypatch.setattr(L, "require_cuda_device", lambda device: None)
-    monkeypatch.setattr(L, "require_cuda", lambda *ts: None)
-    monkeypatch.setattr(L, "load", lambda *a, **k: None)
-    monkeypatch.setattr(L, "launch_count", lambda: 0)
+    cabi_spec.install_spec_backend(monkeypatch)
 
     class _NoEvent:
         def __init__(self, *a, **k):

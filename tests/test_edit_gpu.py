@@ -13,7 +13,8 @@ from tango_b200 import lib as L
 from tango_b200 import parallel, synth
 from tango_b200.pipeline import AudioDiffusion, Tango
 from tango_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
-from test_edit_cpu import case_kwargs, spec_latent_blend
+from cabi_spec import spec_latent_blend
+from test_edit_cpu import case_kwargs
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")

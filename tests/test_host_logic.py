@@ -6,23 +6,20 @@ import numpy as np
 import pytest
 import torch
 
+import cabi_spec
 from oracle import schedulers as osched
 from tango_b200 import ops, synth
 from tango_b200 import schedulers as S
 
 
-def emulate_step(coef, v, s, noise):
-    """The arithmetic of tng_sched_step (elementwise.cu:sched_step_kernel) restated with torch CPU fp32 ops."""
-    c = [coef[i] for i in range(10)]
-    x0 = (c[0] * s + c[1] * v) / c[9]
-    if float(c[8]) > 0:
-        x0 = x0.clamp(-float(c[8]), float(c[8]))
-    out = c[2] * x0 + c[3] * s
-    if float(c[7]) != 0:
-        out = out + c[7] * (c[5] * s + c[6] * v)
-    if noise is not None and float(c[4]) != 0:
-        out = out + c[4] * noise
-    return out
+def spec_step(coef, v, s, noise):
+    """tng_sched_step (latent_step.cu, SchedStep) without CFG on NCHW tensors, through cabi_spec.spec_sched_step."""
+    B, Cc = s.shape[:2]
+    HW = s[0, 0].numel()
+    prev = torch.empty(s.shape)
+    cabi_spec.spec_sched_step(v.reshape(B, Cc, HW).transpose(1, 2).reshape(B * HW, Cc), False, 1.0, s, noise, coef,
+                              prev, None, B=B, Cc=Cc, HW=HW)
+    return prev
 
 
 @pytest.mark.parametrize("n", [10, 100, 200])
@@ -57,12 +54,12 @@ def test_coefficient_tables_bit_exact_vs_oracle(pred):
             v = torch.sin(x * 2 + i)
             nz = torch.randn(x.shape, generator=g)
             ref = o.step(v, t, x, nz if int(t) > 0 else None)
-            got = emulate_step(tab[i], v, x, nz)
+            got = spec_step(tab[i], v, x, nz)
             assert torch.equal(ref, got)
             x = ref
         # last step (t == 0): no noise
         t = o.timesteps[-1]
-        assert torch.equal(o.step(x, t, x), emulate_step(tab[-1], x, x, None))
+        assert torch.equal(o.step(x, t, x), spec_step(tab[-1], x, x, None))
         di = S.DDIMScheduler.from_pretrained(prediction_type=pred)
         di.set_timesteps(n)
         oi = osched.OracleDDIM(**cfg)
@@ -72,8 +69,26 @@ def test_coefficient_tables_bit_exact_vs_oracle(pred):
         for i, t in enumerate(oi.timesteps[:12]):
             v = torch.cos(x * 2 + i)
             ref = oi.step(v, t, x)
-            assert torch.equal(ref, emulate_step(tabi[i], v, x, None))
+            assert torch.equal(ref, spec_step(tabi[i], v, x, None))
             x = ref
+
+
+def test_off_grid_step_keeps_the_grid_table(monkeypatch):
+    """DDPM / DDIM `step` at a timestep outside the grid computes that timestep's row on its own: the grid's
+    coefficient_table() is unchanged, and a later step on the grid still takes its table row."""
+    cabi_spec.install_spec_backend(monkeypatch)     # `step` refuses CPU tensors
+    g = torch.Generator().manual_seed(3)
+    x, v, nz = (torch.randn(2, 8, 4, 4, generator=g) for _ in range(3))
+    for s in (S.DDPMScheduler.from_pretrained(), S.DDIMScheduler.from_pretrained()):
+        s.set_timesteps(10)
+        full = s.coefficient_table().clone()
+        assert 7 not in s.timesteps.tolist()
+        got = s.step(v, 7, x, variance_noise=nz).prev_sample
+        assert torch.equal(got, spec_step(s._coefficients(7), v, x, nz if s._needs_noise(7) else None))
+        assert s.coefficient_table().shape == (10, S.NCOEF) and torch.equal(s.coefficient_table(), full)
+        t = int(s.timesteps[3])
+        got = s.step(v, t, x, variance_noise=nz).prev_sample
+        assert torch.equal(got, spec_step(full[3], v, x, nz if s._needs_noise(t) else None))
 
 
 def test_unet_shapes_and_param_count():
@@ -246,7 +261,7 @@ def test_product_scheduler_tables_meet_reference_loop_constants():
         tab = d.coefficient_table()
         x = x_init.clone()
         for i, t in enumerate(d.timesteps):
-            x = emulate_step(tab[i], model(x, t), x, None)
+            x = spec_step(tab[i], model(x, t), x, None)
         assert abs(x.abs().sum().item() - es) < 1e-2 and abs(x.abs().mean().item() - em) < 1e-3
     for pred, es, em in (("epsilon", 258.9606, 0.3372), ("v_prediction", 202.0296, 0.2631)):
         d = S.DDPMScheduler(**dict(base, prediction_type=pred))
@@ -257,7 +272,7 @@ def test_product_scheduler_tables_meet_reference_loop_constants():
         for i, t in enumerate(d.timesteps):
             res = model(x, t)
             noise = torch.randn(res.shape, generator=g) if int(t) > 0 else None
-            x = emulate_step(tab[i], res, x, noise)
+            x = spec_step(tab[i], res, x, noise)
         assert abs(x.abs().sum().item() - es) < 1e-2 and abs(x.abs().mean().item() - em) < 1e-3
 
 

@@ -19,7 +19,6 @@ import cabi_spec as S
 from tango_b200 import lib as L
 from tango_b200 import ops
 from tango_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
-from test_dpm_solver_cpu import spec_dpm_step
 
 pytestmark = pytest.mark.gpu
 
@@ -808,9 +807,9 @@ def test_dpm_step_bit_exact(cuda, row, layout):
     p_c = None if prev is None else (s_c if alias else prev.cpu().clone())
     m0_c = m0.cpu_clone()
     n_c = None if nin is None else nin.cpu_clone()
-    spec_dpm_step(mo.cpu(), cfg, 3.0, s_c, coef, order, m0_c.buf[0], None if m1 is None else m1.cpu(),
-                  None if m2 is None else m2.cpu(), p_c, None if n_c is None else n_c.view, B=B, Cc=Cc, HW=HW,
-                  split_off=0 if nin is None else nin.split_off)
+    S.spec_dpm_step(mo.cpu(), cfg, 3.0, s_c, coef, order, m0_c.buf[0], None if m1 is None else m1.cpu(),
+                    None if m2 is None else m2.cpu(), p_c, None if n_c is None else n_c.view, B=B, Cc=Cc, HW=HW,
+                    split_off=0 if nin is None else nin.split_off)
     L.dpm_step(mo, cfg, 3.0, sample, poisoned_flat(coef.to(cuda), lead=4), order, m0.buf[0], m1, m2, prev,
                None if nin is None else nin.view, B=B, Cc=Cc, HW=HW, split_off=0 if nin is None else nin.split_off)
     torch.cuda.synchronize()

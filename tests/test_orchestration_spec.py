@@ -21,11 +21,7 @@ CPU = torch.device("cpu")
 
 @pytest.fixture(autouse=True)
 def _spec_backend(monkeypatch):
-    for name, fn in cabi_spec.SPEC.items():
-        monkeypatch.setattr(L, name, fn)
-    monkeypatch.setattr(L, "require_cuda_device", lambda device: None)
-    monkeypatch.setattr(L, "require_cuda", lambda *ts: None)
-    monkeypatch.setattr(L, "load", lambda *a, **k: None)
+    cabi_spec.install_spec_backend(monkeypatch)
 
 
 def rel(a, b):
@@ -180,7 +176,6 @@ def test_inference_loop_orchestration_vs_reference_golden(monkeypatch, precision
     from tango_b200.schedulers import DDPMScheduler
     monkeypatch.setattr(torch.cuda, "Event", _NoEvent)
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
-    monkeypatch.setattr(L, "launch_count", lambda: 0)
     gd = np.load(os.path.join(GOLD, "tiny_inference.npz"))
     cfg = synth.TINY_UNET_CONFIG
     m = AudioDiffusion(unet_config=cfg, precision=precision, use_cuda_graph=False).to(CPU)
@@ -204,7 +199,6 @@ def test_mustango_inference_loop_vs_oracle(monkeypatch):
     from tango_b200.schedulers import DDPMScheduler
     monkeypatch.setattr(torch.cuda, "Event", _NoEvent)
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
-    monkeypatch.setattr(L, "launch_count", lambda: 0)
     cfg = synth.TINY_MUSIC_UNET_CONFIG
     sd = synth.synth_state_dict(synth.unet_param_shapes(cfg), seed=0)
     B, steps, guidance, D = 1, 3, 3.0, cfg["cross_attention_dim"]
@@ -235,7 +229,6 @@ def test_tango_generate_prompt_to_waveform_vs_oracle(monkeypatch):
     from tango_b200.pipeline import Tango
     monkeypatch.setattr(torch.cuda, "Event", _NoEvent)
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
-    monkeypatch.setattr(L, "launch_count", lambda: 0)
     cfg = synth.TINY_UNET_CONFIG
     t = Tango.from_synthetic(unet_config=cfg, device="cpu", precision="split")
     t.model.use_cuda_graph = False
