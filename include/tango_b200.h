@@ -255,6 +255,40 @@ int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guida
                  void* next_in, int64_t ld_in, int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Fused classifier-free guidance + multistep UniPC predictor-corrector update (one HBM pass).
+ * Replaces: models.py:244-249 and UniPCMultistepScheduler.step (scheduling_unipc_multistep.py:490-572:
+ *           convert_model_output :225-278, the UniC corrector :384-488 and the UniP predictor :279-382).
+ * coef = float[18], fp32 scalars computed on the host with the reference's own fp32 op order (device pointer):
+ *   [0..2]   {c_a, c_b, c_d}          conversion of the model output at this step's timestep t_i
+ *   [3..10]  {c_x, c_m, c_b, r_0, r_1, rho_0, rho_1, rho_last}  corrector from s0 = t_{i-1} to t_i
+ *   [11..17] {c_x, c_m, c_b, r_0, r_1, rho_0, rho_1}            predictor from s0 = t_i to t_{i+1}
+ *   with c_x = sigma_t / sigma_s0, c_m = alpha_t * h_phi_1, c_b = alpha_t * B_h (alpha and sigma swapped when the
+ *   solver predicts the noise), r_k = (lambda_{s_k} - lambda_s0) / h and rho the UniC / UniP weights.
+ *   v    = u + guidance * (t - u)  (cfg) or the model output itself
+ *   m    = (c_a * sample + c_b * v) / c_d                                  written to m_cur
+ *   corrector (p = corrector_order >= 1; p = 0 skips it and x = sample):
+ *     D_k  = (m_prev(k+1) - m_prev1) / r_k                                 k < p - 1
+ *     corr = 0 (p = 1), rho_0 * D_0 (p = 2), fma(rho_1, D_1, rho_0 * D_0) (p = 3)
+ *     x    = (c_x * last - c_m * m_prev1) - c_b * (corr + rho_last * (m - m_prev1))      written to last
+ *   predictor (q = predictor_order):
+ *     D_k  = (m_prev(k+1) - m) / r_k                                       k < q - 1
+ *     res  = 0 (q = 1), rho_0 * D_0 (q = 2), fma(rho_1, D_1, rho_0 * D_0) (q = 3)
+ *     prev = (c_x * x - c_m * m) - c_b * res
+ * every other product / sum is one round-to-nearest fp32 op, so prev equals the reference's CPU fp32 result bit for
+ * bit. model_out: fp32 channels-last [(2)B, HW, C] (uncond half first when cfg); sample, m_cur, m_prev1..3 (the
+ * converted outputs of this step and of the 1..3 steps before), last (in: the corrected sample of the previous step;
+ * out: this step's) and prev: fp32 NCHW [B, C, HW]. prev may alias sample; m_cur may alias no history slot it reads.
+ * last may be NULL when p = 0. Also writes next_in: the channels-last bf16 UNet input [(2)B, HW, ld_in] (duplicated
+ * for the CFG halves, hi/lo split at split_off when > 0). TNG_EINVAL as tng_sched_step (required: model_out, sample,
+ * coef, m_cur, and prev or next_in), for p outside 0-3 or q outside 1-3, for a missing history slot among the
+ * max(p, q - 1) it reads or one equal to m_cur, and for a missing last when p > 0.
+ */
+int tng_unipc_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
+                   const float* coef, int32_t corrector_order, int32_t predictor_order, float* m_cur,
+                   const float* m_prev1, const float* m_prev2, const float* m_prev3, float* last, float* prev,
+                   void* next_in, int64_t ld_in, int32_t split_off, int64_t B, int64_t C, int64_t HW, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Latent blend of text-guided editing / inpainting (one HBM pass), run after tng_sched_step / tng_dpm_step.
  * Replaces: the schedulers' add_noise (scheduling_ddpm.py:351-372; DDIM and DPM-Solver use the same formula) and the
  *           masking of StableDiffusionInpaintPipelineLegacy (pipeline_stable_diffusion_inpaint_legacy.py:692-709).

@@ -43,10 +43,10 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     p.add_argument("--output_root", type=str, default="outputs")
     p.add_argument("--exp_id", type=str, default=None, help="Run id (default: unix time; pass one under torchrun)")
     p.add_argument("--precision", default="bf16", choices=["bf16", "split"])
-    p.add_argument("--scheduler", default="ddpm", choices=["ddpm", "ddim", "dpmsolver++"],
-                   help="inference_hf.py uses DDPM; dpmsolver++ samples in 20-25 steps")
-    p.add_argument("--solver_order", type=int, default=2, choices=[1, 2, 3], help="DPM-Solver++ order (--scheduler "
-                   "dpmsolver++ only)")
+    p.add_argument("--scheduler", default="ddpm", choices=["ddpm", "ddim", "dpmsolver++", "unipc"],
+                   help="inference_hf.py uses DDPM; dpmsolver++ samples in 20-25 steps, unipc in 5-10")
+    p.add_argument("--solver_order", type=int, default=2, choices=[1, 2, 3], help="DPM-Solver++ / UniPC order "
+                   "(--scheduler dpmsolver++ or unipc only)")
     p.add_argument("--latent_h", type=int, default=256, help="latent frames: 256 = 10.24 s (reference)")
     p.add_argument("--seed", type=int, default=None, help="torch.manual_seed for reproducible noise")
     return p.parse_args(argv)
@@ -94,6 +94,9 @@ def build_tango(checkpoint: str, device: str, precision: str, scheduler: str, so
         from .schedulers import DPMSolverMultistepScheduler
         # the betas and prediction type of the checkpoint's scheduler_config.json, as diffusers' from_config does
         t.scheduler = DPMSolverMultistepScheduler.from_config(t.scheduler.config, solver_order=solver_order)
+    elif scheduler == "unipc":
+        from .schedulers import UniPCMultistepScheduler
+        t.scheduler = UniPCMultistepScheduler.from_config(t.scheduler.config, solver_order=solver_order)
     return t
 
 

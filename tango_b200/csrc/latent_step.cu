@@ -1,5 +1,5 @@
 // latent_step.cu — the latent updates run between two UNet replays: the DDPM / DDIM step, the multistep DPM-Solver
-// step and the latent blend of editing / inpainting. Each is fused with the CFG combine it reads and the packing of the
+// step, the UniPC predictor-corrector step and the latent blend of editing / inpainting. Each is fused with the CFG combine it reads and the packing of the
 // next UNet input, in one HBM pass. The per-step scalars come from a host-computed coefficient row (device pointer, see
 // tango_b200/schedulers.py); every product and sum is one IEEE round-to-nearest op in the reference's association
 // order, so each update equals the reference's fp32 CPU arithmetic bit for bit.
@@ -103,6 +103,49 @@ struct DpmStep {
   }
 };
 
+// UniPCMultistepScheduler.step (scheduling_unipc_multistep.py:490-572): convert_model_output (:225-278) from the
+// uncorrected sample, written to the history slot m_out; the UniC corrector of order p (:384-488; p = 0: none) from
+// last, m1 = m_{i-1} and the older slots, written back to last; then the UniP predictor of order q (:279-382) from
+// the corrected sample, m_out, m1 and m2. The two-term einsum of the fork is fma(rho_1, D1_1, rho_0 * D1_0).
+struct UniPcStep {
+  static constexpr int kCoefs = 18;
+  const float* sample;
+  int p, q;
+  float* m_out;
+  const float* m1_in;
+  const float* m2_in;
+  const float* m3_in;
+  float* last;
+  __device__ float operator()(const LatentStep& pr, const float* k, const LatentElem& e) const {
+    const float s = sample[e.nchw];
+    const float v = guided_output(pr, e);
+    const float m = __fdiv_rn(__fadd_rn(__fmul_rn(k[0], s), __fmul_rn(k[1], v)), k[2]);
+    m_out[e.nchw] = m;
+    float x = s;
+    if (p > 0) {
+      // x_t_ - c_b * (corr_res + rho_last * (m - m_{i-1})), x_t_ = c_x * last - c_m * m_{i-1}; corr_res = 0 for p = 1
+      const float m1 = m1_in[e.nchw];
+      float corr = 0.f;
+      if (p >= 2) {
+        const float d0 = __fdiv_rn(__fsub_rn(m2_in[e.nchw], m1), k[6]);
+        corr = __fmul_rn(k[8], d0);
+        if (p == 3) corr = __fmaf_rn(k[9], __fdiv_rn(__fsub_rn(m3_in[e.nchw], m1), k[7]), corr);
+      }
+      const float sum = __fadd_rn(corr, __fmul_rn(k[10], __fsub_rn(m, m1)));
+      x = __fsub_rn(__fsub_rn(__fmul_rn(k[3], last[e.nchw]), __fmul_rn(k[4], m1)), __fmul_rn(k[5], sum));
+    }
+    if (last) last[e.nchw] = x;
+    // x_t_ - c_b * pred_res, x_t_ = c_x * x - c_m * m; pred_res = 0 for q = 1
+    float res = 0.f;
+    if (q >= 2) {
+      const float d0 = __fdiv_rn(__fsub_rn(m1_in[e.nchw], m), k[14]);
+      res = __fmul_rn(k[16], d0);
+      if (q == 3) res = __fmaf_rn(k[17], __fdiv_rn(__fsub_rn(m2_in[e.nchw], m), k[15]), res);
+    }
+    return __fsub_rn(__fsub_rn(__fmul_rn(k[11], x), __fmul_rn(k[12], m)), __fmul_rn(k[13], res));
+  }
+};
+
 // The schedulers' add_noise (scheduling_ddpm.py:351-372) and, under a mask, the legacy-inpaint blend
 // (pipeline_stable_diffusion_inpaint_legacy.py:692-709).
 struct LatentBlend {
@@ -191,6 +234,28 @@ extern "C" int tng_dpm_step(const float* model_out, int64_t ld_mo, int32_t cfg, 
                      split_off};
   return launch_latent_step("dpm_step", model_out && sample && m0, p, B, C, HW, DpmStep{sample, order, m0, m1, m2},
                             stream);
+}
+
+extern "C" int tng_unipc_step(const float* model_out, int64_t ld_mo, int32_t cfg, float guidance, const float* sample,
+                              const float* coef, int32_t corrector_order, int32_t predictor_order, float* m_cur,
+                              const float* m_prev1, const float* m_prev2, const float* m_prev3, float* last,
+                              float* prev, void* next_in, int64_t ld_in, int32_t split_off, int64_t B, int64_t C,
+                              int64_t HW, void* stream) {
+  const int p = corrector_order, q = predictor_order;
+  if (p < 0 || p > 3) return set_error(TNG_EINVAL, "unipc_step: corrector order %d is not 0, 1, 2 or 3", p);
+  if (q < 1 || q > 3) return set_error(TNG_EINVAL, "unipc_step: predictor order %d is not 1, 2 or 3", q);
+  // the corrector of order p reads m_{i-1} .. m_{i-p}, the predictor of order q m_{i-1} .. m_{i-q+1}
+  const int depth = p > q - 1 ? p : q - 1;
+  const float* hist[3] = {m_prev1, m_prev2, m_prev3};
+  for (int j = 0; j < depth; ++j) {
+    if (!hist[j]) return set_error(TNG_EINVAL, "unipc_step: orders (%d, %d) need history slot %d", p, q, j + 1);
+    if (hist[j] == m_cur) return set_error(TNG_EINVAL, "unipc_step: m_cur aliases history slot %d", j + 1);
+  }
+  if (p > 0 && !last) return set_error(TNG_EINVAL, "unipc_step: corrector order %d needs last", p);
+  const LatentStep ps{model_out, ld_mo, cfg, guidance, coef, prev, static_cast<__nv_bfloat16*>(next_in), ld_in,
+                      split_off};
+  return launch_latent_step("unipc_step", model_out && sample && m_cur, ps, B, C, HW,
+                            UniPcStep{sample, p, q, m_cur, m_prev1, m_prev2, m_prev3, last}, stream);
 }
 
 extern "C" int tng_latent_blend(const float* x0, const float* noise, const float* mask, int64_t mask_bstride,

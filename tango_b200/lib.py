@@ -25,6 +25,7 @@ SYMBOLS = [
     "tng_transpose_bf16", "tng_sched_step", "tng_timestep_embedding", "tng_linear_f32", "tng_convt_gather",
     "tng_tanh_to_i16", "tng_rmsnorm", "tng_gather_rows", "tng_rel_attention", "tng_stft_frames", "tng_stft_magnitude",
     "tng_log_clamp", "tng_attention_wide", "tng_gemm_plan", "tng_dpm_step", "tng_latent_blend",
+    "tng_unipc_step",
 ]
 
 
@@ -105,6 +106,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
         "tng_transpose_bf16": [vp, i64, i64, i64, i64, vp, i64, vp],
         "tng_sched_step": [vp, i64, i32, f32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
         "tng_dpm_step": [vp, i64, i32, f32, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp],
+        "tng_unipc_step": [vp, i64, i32, f32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64,
+                           vp],
         "tng_latent_blend": [vp, vp, vp, i64, vp, vp, vp, i64, i32, i32, i64, i64, i64, vp],
         "tng_timestep_embedding": [vp, i64, i32, i32, f32, vp, vp],
         "tng_linear_f32": [vp, i64, i64, vp, vp, i64, i32, i32, vp, vp],
@@ -410,6 +413,24 @@ def dpm_step(model_out, cfg, guidance, sample, coef, order, m0, m1, m2, prev, ne
     _call("dpm_step", nbytes, load().tng_dpm_step, model_out.data_ptr(), model_out.stride(0), int(cfg), guidance,
           sample.data_ptr(), coef.data_ptr(), order, m0.data_ptr(), ptr(m1), ptr(m2), ptr(prev), ptr(next_in),
           0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
+
+
+def unipc_step(model_out, cfg, guidance, sample, coef, corrector_order, predictor_order, m_cur, m_prev, last, prev,
+               next_in, *, B, Cc, HW, split_off=0):
+    """tng_unipc_step: CFG combine + conversion to m_cur (written) + UniC corrector of `corrector_order` (0: none) from
+    `last` (read, then overwritten with the corrected sample) + UniP predictor of `predictor_order` (1-3) + packing of
+    the next UNet input. m_prev: the history slots (m_{i-1}, m_{i-2}, m_{i-3}), None where unused; see
+    include/tango_b200.h."""
+    m_prev = tuple(m_prev) + (None,) * (3 - len(m_prev))
+    require_cuda(model_out, sample, coef, m_cur, *m_prev, last, prev, next_in)
+    n = B * Cc * HW
+    p, q = corrector_order, predictor_order
+    reads = max(p, q - 1)
+    nbytes = n * 4 * ((2 if cfg else 1) + 1 + 1 + reads + (2 if p else 0) + (p == 0 and last is not None)
+                      + (prev is not None)) + _next_in_bytes(next_in, n, cfg, split_off)
+    _call("unipc_step", nbytes, load().tng_unipc_step, model_out.data_ptr(), model_out.stride(0), int(cfg), guidance,
+          sample.data_ptr(), coef.data_ptr(), p, q, m_cur.data_ptr(), *(ptr(t) for t in m_prev), ptr(last), ptr(prev),
+          ptr(next_in), 0 if next_in is None else next_in.stride(0), split_off, B, Cc, HW, stream_ptr())
 
 
 def latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW, cfg=False, split_off=0):

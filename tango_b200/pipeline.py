@@ -35,7 +35,7 @@ from . import lib as L
 from . import parallel
 from . import synth
 from .blocks import GraphCache
-from .schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
+from .schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, UniPCMultistepScheduler
 from .stft import TacotronSTFT, wav_to_fbank
 from .t5 import T5EncoderModel
 from .unet import UNet2DConditionModel
@@ -533,6 +533,8 @@ class Tango:
             self.scheduler = DDIMScheduler.from_pretrained(None)
         elif scheduler == "dpmsolver++":   # DPM-Solver++ 2M on the SD-2.1 betas (v-prediction)
             self.scheduler = DPMSolverMultistepScheduler.from_config(self.scheduler.config)
+        elif scheduler == "unipc":         # UniPC-2 bh2 on the SD-2.1 betas (v-prediction)
+            self.scheduler = UniPCMultistepScheduler.from_config(self.scheduler.config)
         if t5_config is not None:
             if t5_config["d_model"] != ucfg["cross_attention_dim"]:
                 raise ValueError("t5_config['d_model'] must equal the UNet's cross_attention_dim")

@@ -1,11 +1,12 @@
-"""DDPM / DDIM / multistep DPM-Solver schedulers with the reference's interface; the update itself runs in one fused
-CUDA kernel.
+"""DDPM / DDIM / multistep DPM-Solver / UniPC schedulers with the reference's interface; the update itself runs in one
+fused CUDA kernel.
 
 Mirrors diffusers' DDPMScheduler / DDIMScheduler as Tango uses them
 (/root/reference/mustango/diffusers/src/diffusers/schedulers/scheduling_ddpm.py:122-349,
 scheduling_ddim.py:132-359; call sites models.py:224-249, tango.py:36): `set_timesteps`, `timesteps`,
 `init_noise_sigma`, `order`, `scale_model_input`, `step(...).prev_sample`, `config`. DPMSolverMultistepScheduler
-(scheduling_dpmsolver_multistep.py:57-535) is the opt-in few-step sampler; its update runs in tng_dpm_step (below).
+(scheduling_dpmsolver_multistep.py:57-535) and UniPCMultistepScheduler (scheduling_unipc_multistep.py:80-572) are the
+opt-in few-step samplers; their updates run in tng_dpm_step and tng_unipc_step (below).
 
 All per-step scalars are computed on the host with the reference's own fp32 torch ops (same association order),
 packed into a [num_steps, 10] coefficient table and shipped to the device once per timestep grid; the kernel
@@ -346,9 +347,66 @@ class DDIMScheduler(_SchedulerBase):
 
 
 NCOEF_DPM = 11
+NCOEF_UNIPC = 18
 
 
-class DPMSolverMultistepScheduler(_SchedulerBase):
+class _MultistepBase(_SchedulerBase):
+    """What the multistep ODE solvers (DPM-Solver, UniPC) share: the VP-type alpha / sigma / lambda schedule, the
+    linspace timestep grid, the conversion of the model output to the solver's prediction, the persistent history
+    slots of the sampling loop and the loop tables whose rows depend on the orders a loop takes."""
+
+    def __init__(self, **cfg):
+        super().__init__(**cfg)
+        # VP-type noise schedule (scheduling_dpmsolver_multistep.py:157-160, scheduling_unipc_multistep.py:162-164)
+        self.alpha_t = torch.sqrt(self.alphas_cumprod)
+        self.sigma_t = torch.sqrt(1 - self.alphas_cumprod)
+        self.lambda_t = torch.log(self.alpha_t) - torch.log(self.sigma_t)
+        self._orders: list = []
+        self._loop_orders: list = []
+
+    def _set_grid(self, num_inference_steps: int):
+        """linspace(0, T-1, n+1) rounded, reversed, last dropped (no steps_offset)."""
+        self.num_inference_steps = num_inference_steps
+        T = self.config["num_train_timesteps"]
+        ts = np.linspace(0, T - 1, num_inference_steps + 1).round()[::-1][:-1].copy().astype(np.int64)
+        self.timesteps = torch.from_numpy(ts)
+
+    def _needs_noise(self, t: int) -> bool:
+        return False   # an ODE solver: nothing is drawn after the initial latents
+
+    def _conversion(self, s0: int, data_prediction: bool):
+        """{c_a, c_b, c_d} with converted = (c_a * sample + c_b * model_output) / c_d at timestep s0: the data
+        prediction x0 (`data_prediction`) or the noise prediction, from the model's `prediction_type`."""
+        one, zero = torch.tensor(1.0), torch.tensor(0.0)
+        a_s0, sg_s0 = self.alpha_t[s0], self.sigma_t[s0]
+        if data_prediction:
+            return {"epsilon": (one, -sg_s0, a_s0), "sample": (zero, one, one),
+                    "v_prediction": (a_s0, -sg_s0, one)}[self.config["prediction_type"]]
+        return {"epsilon": (zero, one, one), "sample": (one, -a_s0, sg_s0),
+                "v_prediction": (sg_s0, a_s0, one)}[self.config["prediction_type"]]
+
+    def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
+        """The coefficient table of a loop entered at timesteps[t_start] (an edit): its rows follow the orders of a
+        loop that starts there, which `_loop_step` then follows. t_start = 0 is the `set_timesteps` table itself."""
+        tab, self._loop_orders = self._table("coef", device, t_start)
+        return tab
+
+    def _table_rows(self, kind: str, t_start: int):
+        if kind != "coef":
+            return super()._table_rows(kind, t_start)
+        orders = self._loop_orders_from(len(self._t_list), t_start)
+        return [self._coefficients_at(i, o) for i, o in enumerate(orders)], orders
+
+    @staticmethod
+    def _history(bufs, sample, count: int) -> list:
+        """`count` persistent NCHW fp32 history slots of the loop, kept with the other buffers of this shape."""
+        hist = bufs.__dict__.setdefault("solver_history", [])
+        while len(hist) < count:
+            hist.append(torch.zeros(sample.shape, device=sample.device, dtype=torch.float32))
+        return hist
+
+
+class DPMSolverMultistepScheduler(_MultistepBase):
     """Multistep DPM-Solver / DPM-Solver++ (scheduling_dpmsolver_multistep.py:57-535), for sampling in 20-25 steps.
 
     The CFG combine, `convert_model_output` and the order-1/2/3 update run as one tng_dpm_step launch. Its per-step
@@ -390,29 +448,18 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
                          prediction_type=prediction_type, thresholding=thresholding,
                          dynamic_thresholding_ratio=dynamic_thresholding_ratio, sample_max_value=sample_max_value,
                          algorithm_type=algorithm_type, solver_type=solver_type, lower_order_final=lower_order_final)
-        # :157-160, VP-type noise schedule
-        self.alpha_t = torch.sqrt(self.alphas_cumprod)
-        self.sigma_t = torch.sqrt(1 - self.alphas_cumprod)
-        self.lambda_t = torch.log(self.alpha_t) - torch.log(self.sigma_t)
         self.model_outputs = [None] * solver_order
         self.lower_order_nums = 0
-        self._orders: list = []
-        self._loop_orders: list = []
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         """:185-206: linspace(0, T-1, n+1) rounded, reversed, last dropped (no steps_offset); resets the history."""
-        self.num_inference_steps = num_inference_steps
-        T = self.config["num_train_timesteps"]
-        ts = np.linspace(0, T - 1, num_inference_steps + 1).round()[::-1][:-1].copy().astype(np.int64)
-        self.timesteps = torch.from_numpy(ts)
+        self._set_grid(num_inference_steps)
+        ts = self.timesteps
         self.model_outputs = [None] * self.config["solver_order"]
         self.lower_order_nums = 0
         self._orders = self._loop_orders_from(len(ts), 0)
         self._loop_orders = self._orders
         self._finish_set_timesteps(device)
-
-    def _needs_noise(self, t: int) -> bool:
-        return False   # an ODE solver: nothing is drawn after the initial latents
 
     def _order_at(self, i: int, n: int, lower_order_nums: int) -> int:
         """The update order :476-487 picks at step index i of n with `lower_order_nums` earlier steps counted."""
@@ -432,22 +479,9 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         full = [self._order_at(i, n, min(i, k)) for i in range(n)]
         return full[:t_start] + [self._order_at(i, n, min(i - t_start, k)) for i in range(t_start, n)]
 
-    def loop_table(self, device, t_start: int = 0) -> torch.Tensor:
-        """The coefficient table of a loop entered at timesteps[t_start] (an edit): its rows come from
-        `_coefficients_at` with the mid-grid orders, which `_loop_step` then follows. t_start = 0 is the
-        `set_timesteps` table itself."""
-        tab, self._loop_orders = self._table("coef", device, t_start)
-        return tab
-
     def order_at(self, i: int) -> int:
         """Order of step i in a loop started by `set_timesteps`."""
         return self._orders[i]
-
-    def _table_rows(self, kind: str, t_start: int):
-        if kind != "coef":
-            return super()._table_rows(kind, t_start)
-        orders = self._loop_orders_from(len(self._t_list), t_start)
-        return [self._coefficients_at(i, o) for i, o in enumerate(orders)], orders
 
     def _coefficients_at(self, i: int, order: int, timestep: Optional[int] = None) -> torch.Tensor:
         """The fp32 scalars of step index i at `order` (:243-281, :305-427, same torch ops in the same order).
@@ -457,16 +491,9 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         tl = self._t_list
         s0 = tl[i] if timestep is None else int(timestep)
         t = 0 if i == len(tl) - 1 else tl[i + 1]   # :463
-        one, zero = torch.tensor(1.0), torch.tensor(0.0)
+        zero = torch.tensor(0.0)
         pp = cfg["algorithm_type"] == "dpmsolver++"
-        pred = cfg["prediction_type"]
-        a_s0, sg_s0 = self.alpha_t[s0], self.sigma_t[s0]
-        if pp:
-            c_a, c_b, c_d = {"epsilon": (one, -sg_s0, a_s0), "sample": (zero, one, one),
-                             "v_prediction": (a_s0, -sg_s0, one)}[pred]
-        else:
-            c_a, c_b, c_d = {"epsilon": (zero, one, one), "sample": (one, -a_s0, sg_s0),
-                             "v_prediction": (sg_s0, a_s0, one)}[pred]
+        c_a, c_b, c_d = self._conversion(s0, pp)
         lambda_t, lambda_s0 = self.lambda_t[t], self.lambda_t[s0]
         alpha_t, alpha_s0 = self.alpha_t[t], self.alpha_t[s0]
         sigma_t, sigma_s0 = self.sigma_t[t], self.sigma_t[s0]
@@ -503,19 +530,12 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
                 c_2 = sigma_t * ((torch.exp(h) - 1.0 - h) / h ** 2 - 0.5)
         return torch.stack([c_a, c_b, c_d, c_s, c_0, c_1, c_2, inv_r0, inv_r1, w_r, inv_r01]).float()
 
-    def _history(self, bufs, sample) -> list:
-        """The loop's `solver_order` persistent NCHW fp32 history slots, kept with the other buffers of this shape."""
-        hist = bufs.__dict__.setdefault("dpm_history", [])
-        while len(hist) < self.config["solver_order"]:
-            hist.append(torch.zeros(sample.shape, device=sample.device, dtype=torch.float32))
-        return hist
-
     def _loop_step(self, i: int, model_out, cfg: bool, guidance: float, sample, noise, coef, next_in, bufs, *, B, Cc,
                    HW, split_off):
         """Step i of AudioDiffusion.inference: the converted output goes to slot i mod k of k = solver_order
         history slots, the previous ones are read from slots i-1 and i-2 mod k."""
-        hist = self._history(bufs, sample)
         k, order = self.config["solver_order"], self._loop_orders[i]
+        hist = self._history(bufs, sample, k)
         m1 = hist[(i - 1) % k] if order >= 2 else None
         m2 = hist[(i - 2) % k] if order >= 3 else None
         L.dpm_step(model_out, cfg, guidance, sample, coef[i], order, hist[i % k], m1, m2, sample, next_in, B=B, Cc=Cc,
@@ -546,6 +566,205 @@ class DPMSolverMultistepScheduler(_SchedulerBase):
         prev = torch.empty_like(sample, dtype=torch.float32)
         L.dpm_step(mo, False, 1.0, sample.contiguous().float(), coef, order, m0, m1, m2, prev, None, B=B, Cc=Cc,
                    HW=H * W)
+        if self.lower_order_nums < k:
+            self.lower_order_nums += 1
+        if not return_dict:
+            return (prev,)
+        return SchedulerOutput(prev_sample=prev)
+
+
+class UniPCMultistepScheduler(_MultistepBase):
+    """Multistep UniPC (scheduling_unipc_multistep.py:80-572): the UniC corrector, then the UniP predictor, per step;
+    built for 5-10 steps.
+
+    The CFG combine, `convert_model_output`, the corrector and the predictor run as one tng_unipc_step launch. Its
+    per-step scalars are computed here with the reference's own fp32 torch ops in the reference's order (the weights
+    rho with its `torch.linalg.solve`) and packed into a [num_steps, 18] table (see include/tango_b200.h for the row):
+    the conversion triple, then {c_x, c_m, c_b, r_0, r_1, rho_0, rho_1, rho_last} of the corrector and
+    {c_x, c_m, c_b, r_0, r_1, rho_0, rho_1} of the predictor. Row i belongs to the (corrector, predictor) orders step i
+    takes in a loop started by `set_timesteps` (or entered at an edit's t_start); `step` keeps the reference's state
+    (`model_outputs`, `timestep_list`, `this_order`, `lower_order_nums`, `last_sample`) and computes the row that state
+    calls for. As in the fork, `solver_type` midpoint / heun / logrho mean bh1. Dynamic thresholding and `solver_p`
+    (another scheduler as the predictor) are not implemented."""
+
+    _ACCEPTED = ("num_train_timesteps", "beta_start", "beta_end", "beta_schedule", "trained_betas", "solver_order",
+                 "prediction_type", "thresholding", "dynamic_thresholding_ratio", "sample_max_value", "predict_x0",
+                 "solver_type", "lower_order_final", "disable_corrector", "solver_p")
+
+    def __init__(self, num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, beta_schedule="linear",
+                 trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                 dynamic_thresholding_ratio=0.995, sample_max_value=1.0, predict_x0=True, solver_type="bh2",
+                 lower_order_final=True, disable_corrector=(), solver_p=None):
+        if thresholding:
+            raise NotImplementedError("thresholding=True (dynamic thresholding) is not implemented for "
+                                      "UniPCMultistepScheduler: it is unsuitable for latent diffusion")
+        if solver_p is not None:
+            raise NotImplementedError("solver_p (another scheduler as the UniPC predictor) is not implemented")
+        if solver_type in ("midpoint", "heun", "logrho"):   # :169-173
+            solver_type = "bh1"
+        elif solver_type not in ("bh1", "bh2"):
+            raise NotImplementedError(f"{solver_type} does is not implemented for {self.__class__}")
+        if solver_order not in (1, 2, 3):
+            raise ValueError(f"solver_order must be 1, 2 or 3, got {solver_order}")
+        if prediction_type not in ("epsilon", "sample", "v_prediction"):
+            raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample`, or"
+                             " `v_prediction` for the UniPCMultistepScheduler.")
+        super().__init__(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                         beta_schedule=beta_schedule, trained_betas=trained_betas, solver_order=solver_order,
+                         prediction_type=prediction_type, thresholding=thresholding,
+                         dynamic_thresholding_ratio=dynamic_thresholding_ratio, sample_max_value=sample_max_value,
+                         predict_x0=predict_x0, solver_type=solver_type, lower_order_final=lower_order_final,
+                         disable_corrector=[int(j) for j in disable_corrector], solver_p=None)
+        self.predict_x0 = predict_x0
+        self.disable_corrector = self.config["disable_corrector"]
+        self.model_outputs = [None] * solver_order
+        self.timestep_list = [None] * solver_order
+        self.lower_order_nums = 0
+        self.this_order = None
+        self.last_sample = None
+        self._rows: dict = {}
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        """:187-211: DPM-Solver's grid; resets `model_outputs`, `lower_order_nums` and `last_sample`."""
+        self._set_grid(num_inference_steps)
+        self.model_outputs = [None] * self.config["solver_order"]
+        self.lower_order_nums = 0
+        self.last_sample = None
+        self._orders = self._loop_orders_from(len(self.timesteps), 0)
+        self._loop_orders = self._orders
+        self._finish_set_timesteps(device)
+
+    def _predictor_order(self, i: int, n: int, lower_order_nums: int) -> int:
+        """The UniP order :550-555 picks at step index i of n with `lower_order_nums` earlier steps counted."""
+        k = self.config["solver_order"]
+        order = min(k, n - i) if self.config["lower_order_final"] else k
+        return min(order, lower_order_nums + 1)
+
+    def _loop_orders_from(self, n: int, t_start: int) -> list:
+        """(corrector, predictor) orders of a loop over steps t_start..n-1 of an n-step grid. The corrector of step i
+        has the order of step i-1's predictor; it is off (0) at the loop's first step, which has no `last_sample`, and
+        where i-1 is in `disable_corrector` (:526-528). Entries before t_start are the full loop's."""
+        k = self.config["solver_order"]
+
+        def run(start):
+            out = []
+            for i in range(start, n):
+                q = self._predictor_order(i, n, min(i - start, k))
+                p = out[-1][1] if i > start and (i - 1) not in self.disable_corrector else 0
+                out.append((p, q))
+            return out
+
+        return run(0)[:t_start] + run(t_start)
+
+    def order_at(self, i: int) -> tuple:
+        """(corrector, predictor) orders of step i in a loop started by `set_timesteps`."""
+        return self._orders[i]
+
+    def _uni_terms(self, s0, t, earlier, order: int, corrector: bool):
+        """(c_x, c_m, c_b, [r_k], [rho]) of a UniC (`corrector`) or UniP update of `order` from s0 to t, `earlier`
+        holding the timesteps of the older history entries, most recent first (:311-379, :415-486, same torch ops in
+        the same order)."""
+        cfg = self.config
+        lambda_t, lambda_s0 = self.lambda_t[t], self.lambda_t[s0]
+        alpha_t, alpha_s0 = self.alpha_t[t], self.alpha_t[s0]
+        sigma_t, sigma_s0 = self.sigma_t[t], self.sigma_t[s0]
+        h = lambda_t - lambda_s0
+        rks = [(self.lambda_t[si] - lambda_s0) / h for si in earlier[:order - 1]]
+        rk_list = list(rks)
+        rks.append(1.0)
+        rks = torch.tensor(rks)
+        hh = -h if self.predict_x0 else h
+        h_phi_1 = torch.expm1(hh)
+        h_phi_k = h_phi_1 / hh - 1
+        factorial_i = 1
+        B_h = hh if cfg["solver_type"] == "bh1" else torch.expm1(hh)
+        R, b = [], []
+        for i in range(1, order + 1):
+            R.append(torch.pow(rks, i - 1))
+            b.append(h_phi_k * factorial_i / B_h)
+            factorial_i *= i + 1
+            h_phi_k = h_phi_k / hh - 1 / factorial_i
+        R = torch.stack(R)
+        b = torch.tensor(b)
+        if corrector:
+            rhos = torch.tensor([0.5]) if order == 1 else torch.linalg.solve(R, b)
+        else:
+            rhos = {1: torch.zeros(0), 2: torch.tensor([0.5])}.get(order)
+            if rhos is None:
+                rhos = torch.linalg.solve(R[:-1, :-1], b[:-1])
+        if self.predict_x0:
+            return sigma_t / sigma_s0, alpha_t * h_phi_1, alpha_t * B_h, rk_list, list(rhos)
+        return alpha_t / alpha_s0, sigma_t * h_phi_1, sigma_t * B_h, rk_list, list(rhos)
+
+    def _row(self, t: int, t_next: int, before: tuple, p: int, q: int) -> torch.Tensor:
+        """The tng_unipc_step row of a step at timestep t towards t_next with corrector order p (0: none) and predictor
+        order q; `before`: the timesteps of the steps before, most recent first."""
+        key = (t, t_next, before, p, q)
+        if key not in self._rows:
+            zero = torch.tensor(0.0)
+            row = list(self._conversion(t, self.predict_x0)) + [zero] * (NCOEF_UNIPC - 3)
+            if p > 0:
+                c_x, c_m, c_b, rk, rho = self._uni_terms(before[0], t, before[1:], p, corrector=True)
+                row[3:6] = [c_x, c_m, c_b]
+                row[6:6 + len(rk)] = rk
+                row[8:8 + len(rho) - 1] = rho[:-1]
+                row[10] = rho[-1]
+            c_x, c_m, c_b, rk, rho = self._uni_terms(t, t_next, before, q, corrector=False)
+            row[11:14] = [c_x, c_m, c_b]
+            row[14:14 + len(rk)] = rk
+            row[16:16 + len(rho)] = rho
+            self._rows[key] = torch.stack([torch.as_tensor(c, dtype=torch.float32) for c in row])
+        return self._rows[key]
+
+    def _coefficients_at(self, i: int, orders: tuple) -> torch.Tensor:
+        tl = self._t_list
+        p, q = orders
+        before = tuple(tl[i - j] for j in range(1, max(p, q - 1) + 1))
+        return self._row(tl[i], 0 if i == len(tl) - 1 else tl[i + 1], before, p, q)
+
+    def _loop_step(self, i: int, model_out, cfg: bool, guidance: float, sample, noise, coef, next_in, bufs, *, B, Cc,
+                   HW, split_off):
+        """Step i of AudioDiffusion.inference: the converted output goes to slot i mod (k + 1) of k + 1 history slots
+        (k = solver_order), so that it never overwrites the m_{i-k} an order-k corrector reads; the corrected sample
+        stays in one persistent buffer for the next step's corrector."""
+        k = self.config["solver_order"]
+        p, q = self._loop_orders[i]
+        hist = self._history(bufs, sample, k + 1)
+        if "unipc_last" not in bufs.__dict__:
+            bufs.unipc_last = torch.zeros(sample.shape, device=sample.device, dtype=torch.float32)
+        m_prev = [hist[(i - j) % (k + 1)] for j in range(1, max(p, q - 1) + 1)]
+        L.unipc_step(model_out, cfg, guidance, sample, coef[i], p, q, hist[i % (k + 1)], m_prev, bufs.unipc_last,
+                     sample, next_in, B=B, Cc=Cc, HW=HW, split_off=split_off)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True, **_unused):
+        """:490-572 for NCHW fp32 CUDA tensors: the corrector (when the state allows it), then the predictor of the
+        order `lower_order_nums` and `lower_order_final` select; the state is updated as the reference does."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the"
+                             " scheduler")
+        L.require_cuda(model_output)   # no CPU fallback
+        t = int(timestep)
+        n = len(self._t_list)
+        i = self._t_index.get(t, n - 1)
+        k = self.config["solver_order"]
+        use_corrector = i > 0 and (i - 1) not in self.disable_corrector and self.last_sample is not None
+        p = self.this_order if use_corrector else 0
+        q = self._predictor_order(i, n, self.lower_order_nums)
+        depth = max(p, q - 1)
+        before = tuple(int(s) for s in self.timestep_list[::-1][:depth])
+        coef = self._row(t, 0 if i == n - 1 else self._t_list[i + 1], before, p, q).to(sample.device)
+        B, Cc, H, W = sample.shape
+        m_cur = torch.empty(sample.shape, device=sample.device, dtype=torch.float32)
+        m_prev = self.model_outputs[::-1][:depth]
+        last = self.last_sample.clone() if p else torch.empty_like(m_cur)
+        mo = model_output.float().permute(0, 2, 3, 1).contiguous().view(B * H * W, Cc)   # channels-last rows
+        prev = torch.empty_like(m_cur)
+        L.unipc_step(mo, False, 1.0, sample.contiguous().float(), coef, p, q, m_cur, m_prev, last, prev, None, B=B,
+                     Cc=Cc, HW=H * W)
+        self.model_outputs = self.model_outputs[1:] + [m_cur]
+        self.timestep_list = self.timestep_list[1:] + [t]
+        self.this_order = q
+        self.last_sample = last
         if self.lower_order_nums < k:
             self.lower_order_nums += 1
         if not return_dict:

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Few-step sampling on the H100: DDPM 200 steps against DPM-Solver++ 2M at 20 and 25 steps, plus the tng_dpm_step
-kernel on its own.
+"""Few-step sampling on the H100: DDPM 200 steps against DPM-Solver++ 2M at 20 and 25 steps and UniPC-2 bh2 at 10 and
+20 steps, plus the tng_dpm_step and tng_unipc_step kernels on their own.
 
     python tools/bench_dpm.py [--rounds 2] [--batch 8] [--kernel-iters 500] [--out FILE]
 
@@ -8,10 +8,12 @@ Workload: the Tango base UNet (seeded synthetic weights), a batch of 8 prompts (
 batch 16), 10.24 s clips (256 x 16 latents), bf16 precision, inputs resident on the device; one pass = the denoising
 loop + VAE decoder + HiFi-GAN. Every configuration is warmed up once, then the configurations are alternated for
 `--rounds` rounds and the median pass is reported as audio-s/s, together with the loop's per-step time (UNet graph
-replay + scheduler kernel). The kernel leg times `--kernel-iters` back-to-back tng_dpm_step launches (order 2, the
-loop's shapes and buffers) with CUDA events and divides the kernel's algorithmic bytes by that time. The card's name
+replay + scheduler kernel). The kernel legs time `--kernel-iters` back-to-back tng_dpm_step launches (order 2) and
+tng_unipc_step launches (order-2 corrector and predictor), at the loop's shapes and buffers, with CUDA events and divide
+each kernel's algorithmic bytes by that time. The card's name
 and power limit are read in the same run. One JSON line goes to stdout (and to --out).
-This measures speed only: the audio quality of 20-25 DPM-Solver++ steps against 200 DDPM steps needs pretrained weights.
+This measures speed only: the audio quality of 20-25 DPM-Solver++ steps or 10-20 UniPC steps against 200 DDPM steps needs
+pretrained weights.
 """
 from __future__ import annotations
 
@@ -54,7 +56,7 @@ def main():
     from tango_b200 import lib as L
     from tango_b200 import synth
     from tango_b200.pipeline import Tango
-    from tango_b200.schedulers import DDPMScheduler, DPMSolverMultistepScheduler
+    from tango_b200.schedulers import DDPMScheduler, DPMSolverMultistepScheduler, UniPCMultistepScheduler
     torch.set_grad_enabled(False)
     dev = torch.device("cuda", 0)
     B, H, W = args.batch, 256, 16
@@ -66,7 +68,9 @@ def main():
     ddpm = DDPMScheduler.from_pretrained()
     configs = {"ddpm_200": (ddpm, 200),
                "dpmsolver++2M_20": (DPMSolverMultistepScheduler.from_config(ddpm.config), 20),
-               "dpmsolver++2M_25": (DPMSolverMultistepScheduler.from_config(ddpm.config), 25)}
+               "dpmsolver++2M_25": (DPMSolverMultistepScheduler.from_config(ddpm.config), 25),
+               "unipc2_bh2_10": (UniPCMultistepScheduler.from_config(ddpm.config), 10),
+               "unipc2_bh2_20": (UniPCMultistepScheduler.from_config(ddpm.config), 20)}
 
     def one_pass(sch, steps):
         gen = torch.Generator(device=dev).manual_seed(1234)
@@ -96,50 +100,61 @@ def main():
     for name in configs:
         out[name]["speedup_vs_ddpm_200"] = out[name]["audio_s_per_s"] / base
 
-    # ---- the kernel alone, at the loop's shapes: CFG halves in, order-2 update, bf16 next input out
+    # ---- the kernels alone, at the loop's shapes: CFG halves in, order-2 update, bf16 next input out
     Cl, HW = 8, H * W
-    sch = DPMSolverMultistepScheduler.from_config(ddpm.config)
-    sch.set_timesteps(25, device=dev)
-    coef = sch.coefficient_table(dev)[5]
+    n = B * Cl * HW
     g = torch.Generator(device=dev).manual_seed(0)
     model_out = torch.randn(2 * B * HW, Cl, device=dev, generator=g)
     sample = torch.randn(B, Cl, H, W, device=dev, generator=g)
-    hist = [torch.randn(B, Cl, H, W, device=dev, generator=g) for _ in range(2)]
+    hist = [torch.randn(B, Cl, H, W, device=dev, generator=g) for _ in range(3)]
+    last = torch.randn(B, Cl, H, W, device=dev, generator=g)
     x_in = torch.zeros(2 * B * HW, Cl, device=dev, dtype=torch.bfloat16)
     prev = torch.empty_like(sample)
-
-    def launch():
-        L.dpm_step(model_out, True, args.guidance, sample, coef, 2, hist[0], hist[1], None, prev, x_in, B=B, Cc=Cl, HW=HW)
-
-    for _ in range(20):
-        launch()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()          # the same launches without the host's per-call cost between them
-    with torch.cuda.graph(graph):
+    dpm = DPMSolverMultistepScheduler.from_config(ddpm.config)
+    dpm.set_timesteps(25, device=dev)
+    dpm_coef = dpm.coefficient_table(dev)[5]
+    uni = UniPCMultistepScheduler.from_config(ddpm.config)
+    uni.set_timesteps(10, device=dev)
+    uni_coef = uni.coefficient_table(dev)[5]
+    assert uni.order_at(5) == (2, 2)
+    kernels = {
+        "dpm_step_kernel": (lambda: L.dpm_step(model_out, True, args.guidance, sample, dpm_coef, 2, hist[0], hist[1],
+                                               None, prev, x_in, B=B, Cc=Cl, HW=HW),
+                            # mo halves, sample, m0, m1, prev; two bf16 input rows
+                            n * 4 * (2 + 1 + 1 + 1 + 1) + n * 2 * 2, "order 2"),
+        "unipc_step_kernel": (lambda: L.unipc_step(model_out, True, args.guidance, sample, uni_coef, 2, 2, hist[0],
+                                                   hist[1:3], last, prev, x_in, B=B, Cc=Cl, HW=HW),
+                              # mo halves, sample, m_i, m_{i-1}, m_{i-2}, last in and out, prev; two bf16 input rows
+                              n * 4 * (2 + 1 + 1 + 2 + 2 + 1) + n * 2 * 2, "corrector order 2, predictor order 2")}
+    kernel_out = {}
+    for name, (launch, nbytes, orders) in kernels.items():
+        for _ in range(20):
+            launch()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()          # the same launches without the host's per-call cost between them
+        with torch.cuda.graph(graph):
+            for _ in range(args.kernel_iters):
+                launch()
+        graph.replay()
+        e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
+        e0.record()
         for _ in range(args.kernel_iters):
             launch()
-    graph.replay()
-    e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
-    e0.record()
-    for _ in range(args.kernel_iters):
-        launch()
-    e1.record()
-    graph.replay()
-    e2.record()
-    torch.cuda.synchronize()
-    us_eager = e0.elapsed_time(e1) * 1e3 / args.kernel_iters
-    us = e1.elapsed_time(e2) * 1e3 / args.kernel_iters
-    n = B * Cl * HW
-    nbytes = n * 4 * (2 + 1 + 1 + 1 + 1) + n * 2 * 2      # mo halves, sample, m0, m1, prev; two bf16 input rows
-    kernel = {"order": 2, "shape": f"B={B} C={Cl} HW={HW}, CFG, bf16 next input", "launches": args.kernel_iters,
-              "us_per_launch": us, "algorithmic_bytes": nbytes, "GB_per_s": nbytes / (us * 1e-6) / 1e9,
-              "us_per_launch_eager": us_eager,
-              "timing": "CUDA events around a graph of back-to-back launches; _eager: the same launches issued one "
-                        "by one from Python (host bound)"}
+        e1.record()
+        graph.replay()
+        e2.record()
+        torch.cuda.synchronize()
+        us_eager = e0.elapsed_time(e1) * 1e3 / args.kernel_iters
+        us = e1.elapsed_time(e2) * 1e3 / args.kernel_iters
+        kernel_out[name] = {"orders": orders, "shape": f"B={B} C={Cl} HW={HW}, CFG, bf16 next input",
+                            "launches": args.kernel_iters, "us_per_launch": us, "algorithmic_bytes": nbytes,
+                            "GB_per_s": nbytes / (us * 1e-6) / 1e9, "us_per_launch_eager": us_eager,
+                            "timing": "CUDA events around a graph of back-to-back launches; _eager: the same launches "
+                                      "issued one by one from Python (host bound)"}
 
     line = {"tool": "bench_dpm", "card": card(), "workload": f"Tango base UNet, batch {B} prompts (UNet batch {2 * B}), "
             f"CFG {args.guidance}, {audio_s:.2f} s clips, 64 synthetic T5 tokens, bf16, device-resident inputs, "
-            "loop + VAE decoder + HiFi-GAN per pass", "rounds": args.rounds, "configs": out, "dpm_step_kernel": kernel}
+            "loop + VAE decoder + HiFi-GAN per pass", "rounds": args.rounds, "configs": out, **kernel_out}
     s = json.dumps(line)
     print(s, flush=True)
     if args.out:
