@@ -111,9 +111,9 @@ typedef struct {
 } tng_gemm_desc;
 
 int tng_conv_gemm(const tng_gemm_desc* d, void* stream);
-/* What tng_conv_gemm would do with this descriptor, without launching: the N tile, the launch mode (always 1 = one CTA
- * per SM on 128 x block_n tiles) and the split-K factor. Used by bench.py to label
- * its per-kernel timings with the instantiation that actually runs. Any output pointer may be NULL. */
+/* What tng_conv_gemm would do with this descriptor, without launching: the N tile, the M tile in `mode` (128, or 256
+ * for large non-GEGLU launches at block_n 160; one CTA per SM on mode x block_n tiles) and the split-K factor. Used by
+ * bench.py to label its per-kernel timings with the instantiation that actually runs. Any output pointer may be NULL. */
 int tng_gemm_plan(const tng_gemm_desc* d, int32_t* block_n, int32_t* mode, int32_t* ksplit);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -3,10 +3,12 @@
 //   384 threads = three warpgroups, warp-specialised. Warpgroup 0 is the producer: one thread feeds the STAGES-deep
 //   shared-memory ring with TMA, cp.async.bulk.tensor 4-D (activations, shifted per tap, OOB zero fill = conv padding)
 //   + 2-D (weights), and hands its registers to the consumers (setmaxnreg). Consumer warpgroup c = 1, 2 owns rows
-//   [64(c-1), 64c) of the 128 x BN output tile and keeps its 64 x BN fp32 accumulator in registers (wgmma.m64nBNk16,
-//   bf16 x bf16 -> fp32, both operands read from shared memory through SWIZZLE_128B descriptors), with one wgmma group
-//   in flight while it waits for the next K block. The ring runs across tile boundaries, so the loads of a CTA's next
-//   tile proceed while the consumers run the epilogue of the current one.
+//   [BM/2 (c-1), BM/2 c) of the BM x BN output tile and keeps its BM/2 x BN fp32 accumulator in registers, one
+//   wgmma.m64nBNk16 per 64 rows (bf16 x bf16 -> fp32, both operands read from shared memory through SWIZZLE_128B
+//   descriptors; the 64-row halves of a 256-row tile share the B descriptor), with one wgmma group in flight while it
+//   waits for the next K block. BM = 128, or 256 with BN = 160 (28 % fewer operand bytes per FLOP than 128 x 160; see
+//   plan_gemm for when). The ring runs across tile boundaries, so the loads of a CTA's next tile proceed while the
+//   consumers run the epilogue of the current one.
 //   Epilogue: every warp moves its 16 rows through an XOR-swizzled 16 x 32 smem transpose, 32 columns at a time, to
 //   fully coalesced global traffic (8 lanes own one 128-byte row segment) with fused bias / per-image vector / residual /
 //   scale / accumulate / activation (SiLU, leaky-ReLU, GEGLU) / bf16 hi-lo split / GroupNorm statistics.
@@ -17,9 +19,7 @@
 
 namespace tng {
 
-constexpr int BM = 128;
 constexpr int BK = 64;  // bf16 elements per 128-byte swizzle row
-constexpr int A_TILE_BYTES = BM * BK * 2;
 constexpr int GEMM_THREADS = 384;
 constexpr int EPI_WARPS = 8;
 constexpr int ES = 4;   // epilogue row slots per lane: a warp's 16 rows = 4 slots x 4 row lanes
@@ -31,7 +31,8 @@ struct KGroupDev {
 struct GemmKernelParams {
   // output pixel grid and M tiling
   int W, H, NB;
-  int bw, bh, bn;
+  int bw, bh, bn;   // M tile = bw x bh x bn output pixels, bm = their product (128 or 256)
+  int bm;
   int tiles_w, tiles_h, tiles_n;
   int m_tiles, n_tiles;
   int Ncols;
@@ -61,8 +62,9 @@ struct GemmKernelParams {
   long long stats_hw;
 };
 
-template <int BN>
+template <int BN, int BM>
 struct GemmCfg {
+  static constexpr int A_TILE_BYTES = BM * BK * 2;
   static constexpr int B_TILE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
   static constexpr int EPI_BYTES = EPI_WARPS * 16 * 32 * 4;  // per warp: 16 x 32 fp32 swizzled transpose tile
@@ -342,13 +344,18 @@ __device__ __forceinline__ int tile_kiters(const GemmKernelParams& p, int tile) 
   return (sp + 1) * p.total_kiters / p.ksplit - sp * p.total_kiters / p.ksplit;
 }
 
-template <int BN>
+template <int BN, int BM>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant__ CUtensorMap amap1,
                const __grid_constant__ CUtensorMap amap2, const __grid_constant__ CUtensorMap amap3,
                const __grid_constant__ CUtensorMap bmap, const __grid_constant__ GemmKernelParams p) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, BM>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int A_TILE_BYTES = Cfg::A_TILE_BYTES;
+  constexpr int MH = BM / 128;   // 64-row accumulator blocks per consumer warpgroup
+  // register split (128 x 24 + 256 x 240 <= 64K): 256-row tiles keep 160 accumulators per consumer thread, and the
+  // producer's one thread fits in 24 registers
+  constexpr int PRODUCER_REGS = BM == 256 ? 24 : 40, CONSUMER_REGS = BM == 256 ? 240 : 232;
   extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B tiles need 1024-byte alignment (checked below)
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_TILE_BYTES;
@@ -380,7 +387,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
   if (wg == 0) {
     // ===================================================== TMA producer: the ring items of this CTA are its work items'
     // K blocks in order; item j lives in slot j % STAGES
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (tid == 0) {
       uint32_t n_loaded = 0;
       for (int tile = work0; tile < total_tiles; tile += work_stride) {
@@ -403,42 +410,52 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
     }
     return;
   }
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<CONSUMER_REGS>();
 
   // ===================================================== main loop + epilogue (consumer warpgroups 1 and 2)
   const int cw = warp - 4;                         // consumer warp 0..7
   float* st = sEpi + cw * (16 * 32);
-  const int wr = 16 * cw;                          // first tile row of this warp
-  const uint32_t a_off = static_cast<uint32_t>(wg - 1) * (64 * 128);   // rows [64 (wg-1), 64 wg) of the A tile
+  // first tile row of this warp in each 64-row block of its warpgroup: wr0 + 64 h, h < MH (the wgmma accumulator
+  // layout gives warp i of a warpgroup rows [16 i, 16 i + 16) of every m64 block)
+  const int wr0 = (BM / 2) * (wg - 1) + 16 * (cw & 3);
+  const uint32_t a_off = static_cast<uint32_t>(wg - 1) * (BM / 2 * 128);   // rows [BM/2 (wg-1), BM/2 wg) of the A tile
   const bool release = (tid & 127) == 0;           // the thread that arrives on the empty barriers for its warpgroup
-  const int mode = (p.res ? 1 : 0) | (p.out_f32 ? 2 : 0) | (p.out_bf16 ? 4 : 0);
-  const bool geglu = (p.act == TNG_ACT_GEGLU || p.act == TNG_ACT_GEGLU_TANH);
   uint32_t n_used = 0;                             // ring items consumed so far
-  float acc[BN / 2];
+  float acc[MH][BN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int h = 0; h < MH; ++h)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
   for (int tile = work0; tile < total_tiles; tile += work_stride) {
     const int nk = tile_kiters(p, tile);
     for (int ki = 0; ki < nk; ++ki) {
       const int slot = static_cast<int>(n_used % STAGES);
       mbar_wait(&full_bar[slot], (n_used / STAGES) & 1);
-      const uint64_t ad = wgmma_desc_sw128(smem_u32(sA + slot * A_TILE_BYTES) + a_off, 16, 1024);
+      const uint32_t sa = smem_u32(sA + slot * A_TILE_BYTES) + a_off;
       const uint64_t bd = wgmma_desc_sw128(smem_u32(sB + slot * Cfg::B_TILE_BYTES), 16, 1024);
-      fence_regs(acc);
+#pragma unroll
+      for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, ad + 2 * k, bd + 2 * k, (ki > 0 || k > 0) ? 1u : 0u);
+      for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+        for (int h = 0; h < MH; ++h)
+          wgmma_ss<BN>(acc[h], wgmma_desc_sw128(sa + h * (64 * 128), 16, 1024) + 2 * k, bd + 2 * k,
+                       (ki > 0 || k > 0) ? 1u : 0u);
       wgmma_commit();
-      fence_regs(acc);
+#pragma unroll
+      for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
       if (ki > 0) {
         wgmma_wait<1>();   // the previous K block's wgmma are complete: release its slot
-        fence_regs(acc);
+#pragma unroll
+        for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
         mbar_arrive_if(&empty_bar[(n_used - 1) % STAGES], release);
       }
       ++n_used;
     }
     wgmma_wait<0>();
-    fence_regs(acc);
+#pragma unroll
+    for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
     mbar_arrive_if(&empty_bar[(n_used - 1) % STAGES], release);
 
     // ---- epilogue: rows of a tile are consecutive output rows; valid rows form a prefix (see host tiling)
@@ -448,45 +465,82 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap0, const __grid_constant_
     else if (p.bn == 1) nvalid = min(p.bh, p.H - w.h0) * p.bw;
     else nvalid = min(p.bn, p.NB - w.n0) * p.bh * p.bw;
     const EpiTile t{(static_cast<long long>(w.n0) * p.H + w.h0) * p.W + w.w0, w.n0, nvalid, w.tn, w.sp};
-    if (geglu) {
-      if constexpr (BN == 128 || BN == 256) {   // the host only selects these N tiles for GEGLU
-        if (p.act == TNG_ACT_GEGLU_TANH) {   // T5 front-end (small): one general instantiation
-          if (p.split_off > 0) epi_tile_geglu<BN, false, true, true>(p, st, acc, t, wr, lane);
-          else epi_tile_geglu<BN, false, false, true>(p, st, acc, t, wr, lane);
-        } else if (p.split_off > 0) epi_tile_geglu<BN, false, true, false>(p, st, acc, t, wr, lane);
-        else if (nvalid == BM) epi_tile_geglu<BN, true, false, false>(p, st, acc, t, wr, lane);
-        else epi_tile_geglu<BN, false, false, false>(p, st, acc, t, wr, lane);
+    const int mode = (p.res ? 1 : 0) | (p.out_f32 ? 2 : 0) | (p.out_bf16 ? 4 : 0);
+    const bool geglu = (p.act == TNG_ACT_GEGLU || p.act == TNG_ACT_GEGLU_TANH);
+    const bool full = p.fast_epi && p.ksplit == 1 && nvalid == BM && (w.tn + 1) * BN <= p.Ncols;
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+      const int wr = wr0 + 64 * h;
+      if (geglu) {
+        if constexpr (BM == 128 && (BN == 128 || BN == 256)) {   // the host only selects these tiles for GEGLU
+          if (p.act == TNG_ACT_GEGLU_TANH) {   // T5 front-end (small): one general instantiation
+            if (p.split_off > 0) epi_tile_geglu<BN, false, true, true>(p, st, acc[h], t, wr, lane);
+            else epi_tile_geglu<BN, false, false, true>(p, st, acc[h], t, wr, lane);
+          } else if (p.split_off > 0) epi_tile_geglu<BN, false, true, false>(p, st, acc[h], t, wr, lane);
+          else if (nvalid == BM) epi_tile_geglu<BN, true, false, false>(p, st, acc[h], t, wr, lane);
+          else epi_tile_geglu<BN, false, false, false>(p, st, acc[h], t, wr, lane);
+        }
+      } else if (full) {
+        switch (mode) {
+          case 2: epi_tile<BN, EPI_FULL, 2>(p, st, acc[h], t, wr, lane); break;
+          case 3: epi_tile<BN, EPI_FULL, 3>(p, st, acc[h], t, wr, lane); break;
+          case 4: epi_tile<BN, EPI_FULL, 4>(p, st, acc[h], t, wr, lane); break;
+          case 5: epi_tile<BN, EPI_FULL, 5>(p, st, acc[h], t, wr, lane); break;
+          case 6: epi_tile<BN, EPI_FULL, 6>(p, st, acc[h], t, wr, lane); break;
+          default: epi_tile<BN, EPI_FULL, 7>(p, st, acc[h], t, wr, lane); break;
+        }
+      } else if (p.fast_epi) {
+        epi_tile<BN, EPI_VEC, 7>(p, st, acc[h], t, wr, lane);
+      } else if constexpr (BM == 128) {   // 256-row tiles: 16-byte aligned operands only (host)
+        epi_tile<BN, EPI_SCALAR, 7>(p, st, acc[h], t, wr, lane);
       }
-    } else if (p.fast_epi && p.ksplit == 1 && nvalid == BM && (w.tn + 1) * BN <= p.Ncols) {
-      switch (mode) {
-        case 2: epi_tile<BN, EPI_FULL, 2>(p, st, acc, t, wr, lane); break;
-        case 3: epi_tile<BN, EPI_FULL, 3>(p, st, acc, t, wr, lane); break;
-        case 4: epi_tile<BN, EPI_FULL, 4>(p, st, acc, t, wr, lane); break;
-        case 5: epi_tile<BN, EPI_FULL, 5>(p, st, acc, t, wr, lane); break;
-        case 6: epi_tile<BN, EPI_FULL, 6>(p, st, acc, t, wr, lane); break;
-        default: epi_tile<BN, EPI_FULL, 7>(p, st, acc, t, wr, lane); break;
-      }
-    } else if (p.fast_epi) {
-      epi_tile<BN, EPI_VEC, 7>(p, st, acc, t, wr, lane);
-    } else {
-      epi_tile<BN, EPI_SCALAR, 7>(p, st, acc, t, wr, lane);
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-template <int BN>
+template <int BN, int BM = 128>
 static int launch_gemm(const CUtensorMap* am, const CUtensorMap& bm, const GemmKernelParams& p, cudaStream_t st) {
-  using Cfg = GemmCfg<BN>;
-  const int rc = set_max_dynamic_smem<gemm_tc_kernel<BN>>(Cfg::SMEM_BYTES, "gemm_tc");
+  using Cfg = GemmCfg<BN, BM>;
+  const int rc = set_max_dynamic_smem<gemm_tc_kernel<BN, BM>>(Cfg::SMEM_BYTES, "gemm_tc");
   if (rc) return rc;
   const int work = p.m_tiles * p.n_tiles * p.ksplit;
   const int grid = work < num_sms() ? work : num_sms();
-  gemm_tc_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(am[0], am[1], am[2], am[3], bm, p);
+  gemm_tc_kernel<BN, BM><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(am[0], am[1], am[2], am[3], bm, p);
   return check_launch("gemm_tc");
 }
 
 static bool is_pow2(long long x) { return x > 0 && (x & (x - 1)) == 0; }
+
+// M tile = bw x bh x bn output pixels with product bm (a power of two), each box dimension <= bm <= 256 (the TMA box
+// limit): whole rows of the output grid when W >= bm, else whole images' worth of rows, so that the rows of a tile are
+// consecutive output rows and its valid rows a prefix. False when the grid does not allow this tiling.
+static bool tile_m(const tng_gemm_desc* d, int bm, GemmKernelParams& p) {
+  if (d->W >= bm || d->H == 1) {
+    p.bw = bm; p.bh = 1; p.bn = 1;
+  } else {
+    if (!is_pow2(d->W)) return false;
+    p.bw = d->W;
+    const int rem = bm / p.bw;
+    if (d->H >= rem) {
+      p.bh = rem; p.bn = 1;
+    } else {
+      if (!is_pow2(d->H)) return false;
+      p.bh = d->H; p.bn = rem / p.bh;
+    }
+  }
+  p.tiles_w = (d->W + p.bw - 1) / p.bw;
+  p.tiles_h = (d->H + p.bh - 1) / p.bh;
+  p.tiles_n = (d->NB + p.bn - 1) / p.bn;
+  p.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  p.bm = bm;
+  return true;
+}
+
+// every M tile of the tiling in p is full
+static bool full_m_tiles(const tng_gemm_desc* d, const GemmKernelParams& p) {
+  return (p.bh == 1 && p.bn == 1) ? (d->W % p.bw == 0) : (p.bn == 1 ? (d->H % p.bh == 0) : (d->NB % p.bn == 0));
+}
 
 }  // namespace tng
 
@@ -504,24 +558,10 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
 
   memset(&p, 0, sizeof(p));
   p.W = d->W; p.H = d->H; p.NB = d->NB;
-  // M tile = bw x bh x bn output pixels (product 128)
-  if (d->W >= BM || d->H == 1) {
-    p.bw = BM; p.bh = 1; p.bn = 1;
-  } else {
+  if (!tile_m(d, 128, p)) {
     if (!is_pow2(d->W)) return set_error(TNG_EINVAL, "W=%d < 128 must be a power of two", d->W);
-    p.bw = d->W;
-    const int rem = BM / p.bw;
-    if (d->H >= rem) {
-      p.bh = rem; p.bn = 1;
-    } else {
-      if (!is_pow2(d->H)) return set_error(TNG_EINVAL, "H=%d (W=%d) must be a power of two when W*H < 128", d->H, d->W);
-      p.bh = d->H; p.bn = rem / p.bh;
-    }
+    return set_error(TNG_EINVAL, "H=%d (W=%d) must be a power of two when W*H < 128", d->H, d->W);
   }
-  p.tiles_w = (d->W + p.bw - 1) / p.bw;
-  p.tiles_h = (d->H + p.bh - 1) / p.bh;
-  p.tiles_n = (d->NB + p.bn - 1) / p.bn;
-  p.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   p.Ncols = (int)d->Ncols;
 
   int bn_tile = d->block_n;
@@ -599,8 +639,19 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
       return set_error(TNG_EINVAL, "gn_stats without an fp32 output needs a plain bf16 output (no activation, no hi/lo split)");
   }
 
-  const bool full_m = (p.bh == 1 && p.bn == 1) ? (d->W % BM == 0) : (p.bn == 1 ? (d->H % p.bh == 0) : (d->NB % p.bn == 0));
   if (p.ksplit > 1 && !p.fast_epi) p.ksplit = 1;
+  // 256-row tiles draw 28 % fewer operand bytes from L2 per FLOP than 128 x 160, but a CTA's epilogue covers twice the
+  // rows and a launch has half the work items. On one H100 SXM (700 W) that pays for long reductions only: 3x3
+  // convolutions with >= 1280 input channels gain up to 5 %; short-K linears (K = 320 / 640) with an fp32 residual lose
+  // 6-12 % and the level-0 3x3 convolution (K = 2880) 3 % (DESIGN.md section 7). So: non-GEGLU (GEGLU's epilogue works
+  // on 128 x 256 tiles), not split-K, 16-byte aligned epilogue operands, >= 64 K blocks, and at least half a wave of
+  // 256-row work items; with fused statistics only when every 256-row tile is full.
+  if (bn_tile == 160 && p.ksplit == 1 && p.fast_epi && p.total_kiters >= 64 && d->act != TNG_ACT_GEGLU &&
+      d->act != TNG_ACT_GEGLU_TANH) {
+    GemmKernelParams q = p;
+    if (tile_m(d, 256, q) && 2LL * q.m_tiles * p.n_tiles >= num_sms() && (!d->gn_stats || full_m_tiles(d, q))) p = q;
+  }
+  const bool full_m = full_m_tiles(d, p);
   // GroupNorm statistics ride in the epilogue when every tile is full (the lean epilogue path), the warp's 16 rows lie
   // in one image and the output is written exactly once; otherwise a separate pass over the output follows the GEMM
   bool stats_after = false;
@@ -622,7 +673,7 @@ extern "C" int tng_gemm_plan(const tng_gemm_desc* d, int32_t* block_n, int32_t* 
   const int rc = plan_gemm(d, p, bn_tile, stats_after);
   if (rc != TNG_OK) return rc;
   if (block_n) *block_n = bn_tile;
-  if (mode) *mode = 1;
+  if (mode) *mode = p.bm;
   if (ksplit) *ksplit = p.ksplit;
   return TNG_OK;
 }
@@ -642,7 +693,7 @@ extern "C" int tng_conv_gemm(const tng_gemm_desc* d, void* stream) {
     if (v.C % 8 != 0) return set_error(TNG_EINVAL, "view %d: C=%lld must be a multiple of 8", i, (long long)v.C);
     uint64_t dims[4] = {(uint64_t)v.C, (uint64_t)v.W, (uint64_t)v.H, (uint64_t)v.NB};
     uint64_t strides[3] = {(uint64_t)v.s_w * 2, (uint64_t)v.s_h * 2, (uint64_t)v.s_n * 2};
-    uint32_t box[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
+    uint32_t box[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};   // bm x BK
     int rc = encode_tmap_bf16(&am[i], v.ptr, 4, dims, strides, box);
     if (rc) return rc;
   }
@@ -665,7 +716,7 @@ extern "C" int tng_conv_gemm(const tng_gemm_desc* d, void* stream) {
     case 32: rc = launch_gemm<32>(am, bm, p, st); break;
     case 64: rc = launch_gemm<64>(am, bm, p, st); break;
     case 128: rc = launch_gemm<128>(am, bm, p, st); break;
-    case 160: rc = launch_gemm<160>(am, bm, p, st); break;
+    case 160: rc = p.bm == 256 ? launch_gemm<160, 256>(am, bm, p, st) : launch_gemm<160>(am, bm, p, st); break;
     case 256: rc = launch_gemm<256>(am, bm, p, st); break;
     default: return set_error(TNG_EINVAL, "block_n=%d unsupported", bn_tile);
   }

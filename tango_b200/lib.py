@@ -281,7 +281,7 @@ def conv_gemm(views: Sequence[View], groups: Sequence[tuple], weight: torch.Tens
         flops = 2.0 * W * H * NB * weight.shape[0] * k_alg
         bn, mode, ks = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         check(lib.tng_gemm_plan(C.byref(d), C.byref(bn), C.byref(mode), C.byref(ks)), "tng_gemm_plan")
-        fam = f"gemm_tc<{bn.value}" + (",splitk>" if ks.value > 1 else ">")
+        fam = f"gemm_tc<{bn.value}" + (",splitk>" if ks.value > 1 else ",m256>" if mode.value == 256 else ">")
         PROF.timed(fam, flops, 0, lambda: check(lib.tng_conv_gemm(C.byref(d), stream_ptr()), "tng_conv_gemm"))
         return
     check(lib.tng_conv_gemm(C.byref(d), stream_ptr()), "tng_conv_gemm")
