@@ -26,7 +26,7 @@ def _gather_view(v, n_idx, h_idx, w_idx, c0, nk):
     flat = v.t.reshape(-1).double()
     ok = (h_idx >= 0) & (h_idx < v.H) & (w_idx >= 0) & (w_idx < v.W) & (n_idx >= 0) & (n_idx < v.NB)
     base = v.off + n_idx.clamp(0, v.NB - 1) * v.s_n + h_idx.clamp(0, v.H - 1) * v.s_h + w_idx.clamp(0, v.W - 1) * v.s_w
-    c = c0 + torch.arange(nk)
+    c = c0 + torch.arange(nk, device=flat.device)
     c_ok = c < v.C
     idx = base[:, None] + c.clamp(max=max(v.C - 1, 0))[None, :]
     vals = flat[idx.clamp(0, flat.numel() - 1)]
@@ -37,15 +37,16 @@ def spec_conv_gemm(views, groups, weight, W, H, NB, *, bias=None, rowvec=None, r
                    out_f32=None, out_bf16=None, act=ACT_NONE, act_param=0.0, split_off=0, block_n=0, rowvec_ld=0,
                    gn_stats=None, stats_hw=0, **_):
     rows = NB * H * W
-    r = torch.arange(rows)
+    dev = weight.device
+    r = torch.arange(rows, device=dev)
     n_idx, h_idx, w_idx = r // (H * W), (r // W) % H, r % W
     Ncols, Ktot = weight.shape
     wd = weight.double()
-    acc = torch.zeros(rows, Ncols, dtype=torch.float64)
+    acc = torch.zeros(rows, Ncols, dtype=torch.float64, device=dev)
     for (vi, a_c0, dw, dh, b_k0, nkb) in groups:
         nk = nkb * BK
         a = _gather_view(views[vi], n_idx, h_idx + dh, w_idx + dw, a_c0, nk)
-        b = torch.zeros(Ncols, nk, dtype=torch.float64)
+        b = torch.zeros(Ncols, nk, dtype=torch.float64, device=dev)
         kmax = max(0, min(nk, Ktot - b_k0))
         b[:, :kmax] = wd[:, b_k0:b_k0 + kmax]
         acc += a @ b.t()
@@ -219,9 +220,9 @@ def spec_transpose_bf16(x, B, R, Cc, y):
 def spec_convt_gather(Y, B, Lin, ktaps, Cout, stride, pad, Lout, bias, y):
     """ConvTranspose1d overlap-add: y[b, l, :] = bias + sum over (q, t) with q*stride + t - pad == l of Y[b, q, t, :]."""
     Yv = Y.reshape(B, Lin, ktaps, Cout).double()
-    out = torch.zeros(B, Lout, Cout, dtype=torch.float64)
+    out = torch.zeros(B, Lout, Cout, dtype=torch.float64, device=Y.device)
     for t in range(ktaps):
-        l = torch.arange(Lin) * stride + t - pad
+        l = torch.arange(Lin, device=Y.device) * stride + t - pad
         ok = (l >= 0) & (l < Lout)
         out[:, l[ok], :] += Yv[:, ok, t, :]
     if bias is not None:
@@ -315,7 +316,7 @@ def spec_latent_blend(x0, noise, mask, coef, sample, next_in=None, *, B, Cc, HW,
 def spec_stft_frames(y, pad, hi, lo):
     """Reflect padding (no edge repeat) by `pad` on both sides, bf16 hi / lo planes, zero beyond T + 2 pad."""
     B, T = y.shape
-    z = torch.zeros(B, hi.shape[1])
+    z = torch.zeros(B, hi.shape[1], device=y.device)
     z[:, :T + 2 * pad] = F.pad(y.float().view(B, 1, T), (pad, pad), mode="reflect").view(B, -1)
     h = z.to(torch.bfloat16)
     hi.copy_(h)

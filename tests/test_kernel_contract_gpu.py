@@ -31,6 +31,18 @@ U32 = 2.0 ** -24  # fp32 unit round-off
 GEMM_GAMMA = 2.0 ** -16
 
 
+def gemm_gamma(k: int) -> float:
+    """GEMM_GAMMA for a reduction of k products, long ones included. The sqrt(k) argument above needs products of
+    random sign; a sum whose products share their sign (softmax P times a value column with a non-zero mean: the
+    split-mode VAE attention, K = 3 x 4096) grows its partial sums steadily, and so does the rounding error. Worst case:
+    wgmma adds one k-step of 16 products to the fp32 accumulator per instruction, and an update rounded in either
+    direction (the tensor core need not round to nearest) errs by at most one ulp, 2u of a partial sum whose magnitude is
+    at most sum |a_k b_k|: (k / 16) * 2^-23 = k * 2^-27 of that sum. Below k = 2048 that is within GEMM_GAMMA; the
+    UNet's 1280-channel 3 x 3 convolution (k = 11 520) gets 2^-13.5, its split form (3 x 11 520) 2^-11.9. On an H100
+    80GB HBM3 (700 W power limit) the k = 12 288 P V product exceeds the fixed 2^-16 bound by a factor of 1.22."""
+    return max(GEMM_GAMMA, k * 2.0 ** -27)
+
+
 def bf(x):
     return x.to(torch.bfloat16)
 
