@@ -101,11 +101,13 @@ typedef struct {
   int32_t split_off;   /* 0 = off */
   int32_t block_n;     /* N tile: 0 = auto; one of 32, 64, 128, 160, 256 */
   /* GroupNorm statistics of the output for the norm that consumes it (resnet.py:555,581; transformer_2d.py:253):
-   * gn_stats[(img * Ncols + n) * 2 + {0, 1}] += sum / sum of squares of x[:, n] (the fp32 epilogue value, before any
-   * rounding; a plain bf16 output without an fp32 one is allowed) over the stats_hw rows of image
+   * gn_stats[(img * Ncols + n) * 2 + {0, 1}] += sum / sum of squares of x[:, n] (the stored value: the fp32 output, or
+   * without one the bf16 output, which must then be plain: no activation, no hi/lo split) over the stats_hw rows of image
    * img = row / stats_hw (fp64 accumulators the caller zeroes; per CHANNEL, so that any grouping - also across the
    * channel concat of a skip connection - is a sum of entries). Emitted from the epilogue of the producing GEMM when
-   * every tile is full, otherwise by a pass over the output that follows it in the stream. NULL = off. */
+   * every tile is full, otherwise by a pass over the output that follows it in the stream, which needs Ncols % 4 == 0
+   * and a stored output with ld % 4 == 0 at an 8-byte aligned address (TNG_EINVAL before any launch otherwise).
+   * NULL = off. */
   double* gn_stats;
   int64_t stats_hw;
 } tng_gemm_desc;

@@ -56,7 +56,7 @@ struct GemmKernelParams {
   float act_param;
   int split_off;
   int fast_epi;  // Ncols % 4 == 0 and every epilogue row stride and base allows 16-byte vector access
-  // GroupNorm statistics of the fp32 output, emitted from the epilogue (full-tile launches only, see the host side):
+  // GroupNorm statistics of the stored output, emitted from the epilogue (full-tile launches only, see the host side):
   // col_stats[(img * Ncols + col) * 2 + {0, 1}] += sum / sum of squares over the rows of image img = row / stats_hw
   double* col_stats;
   long long stats_hw;
@@ -80,6 +80,7 @@ enum EpiShape { EPI_SCALAR, EPI_VEC, EPI_FULL };
 
 __device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
 __device__ __forceinline__ float4 scale4(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
+__device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
 // act_f over a chunk, with the activation fixed at compile time
 template <int ACT>
@@ -239,12 +240,16 @@ __device__ __forceinline__ void epi_tile(const GemmKernelParams& p, float* st, c
       // Column sums of this warp's 16 rows x 32 columns (all rows belong to image simg): 4 rows in registers,
       // then across the four row-lanes (lane bits 3 and 4); lanes 0..7 hold the totals of their 4 columns and add
       // them to the fp64 per-(image, channel) accumulators — fp32 partials over 16 values, fp64 across tiles.
+      // Without an fp32 output they are the statistics of the stored bf16 values (a plain bf16 output: host check),
+      // as the after-pass computes them.
       float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
 #pragma unroll
       for (int i = 0; i < ES; ++i) {
-        s0 += a[i].x; s1 += a[i].y; s2 += a[i].z; s3 += a[i].w;
-        q0 = fmaf(a[i].x, a[i].x, q0); q1 = fmaf(a[i].y, a[i].y, q1);
-        q2 = fmaf(a[i].z, a[i].z, q2); q3 = fmaf(a[i].w, a[i].w, q3);
+        float4 v = a[i];
+        if constexpr (!(MODE & 2)) v = make_float4(bf16_round(v.x), bf16_round(v.y), bf16_round(v.z), bf16_round(v.w));
+        s0 += v.x; s1 += v.y; s2 += v.z; s3 += v.w;
+        q0 = fmaf(v.x, v.x, q0); q1 = fmaf(v.y, v.y, q1);
+        q2 = fmaf(v.z, v.z, q2); q3 = fmaf(v.w, v.w, q3);
       }
 #pragma unroll
       for (int o = 8; o <= 16; o <<= 1) {
@@ -660,6 +665,13 @@ static int plan_gemm(const tng_gemm_desc* d, GemmKernelParams& p, int& bn_tile_o
                        (d->stats_hw % 16 == 0) && d->act != TNG_ACT_GEGLU && d->act != TNG_ACT_GEGLU_TANH;
     if (fused) { p.col_stats = d->gn_stats; p.stats_hw = d->stats_hw; }
     else stats_after = true;
+    // the after-pass (launch_col_stats) reads the stored output 4 columns at a time: refuse before the GEMM runs what
+    // it would refuse after the GEMM has written the output
+    const void* so = d->out_f32 ? static_cast<const void*>(d->out_f32) : d->out_bf16;
+    const long long sld = d->out_f32 ? d->ld_f32 : d->ld_bf16;
+    if (stats_after && (d->Ncols % 4 || sld % 4 || (reinterpret_cast<uintptr_t>(so) & 7)))
+      return set_error(TNG_EINVAL, "gn_stats after the GEMM needs Ncols %% 4 == 0 and a stored output with ld %% 4 == 0, "
+                       "8-byte aligned (Ncols=%lld ld=%lld)", (long long)d->Ncols, sld);
   }
   bn_tile_out = bn_tile;
   stats_after_out = stats_after;

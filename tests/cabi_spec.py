@@ -65,8 +65,9 @@ def spec_conv_gemm(views, groups, weight, W, H, NB, *, bias=None, rowvec=None, r
         if accumulate:        # the accumulated value is also what the bf16 output (if any) is derived from
             y = y + out_f32[:, :Ncols].double()
         out_f32[:, :Ncols] = y.float()
-    if gn_stats is not None:   # per-(image, channel) sums of the fp32 epilogue value are ADDED to the accumulators
-        yi = y.float().double().view(rows // stats_hw, stats_hw, Ncols)
+    if gn_stats is not None:   # per-(image, channel) sums of the stored value are ADDED to the accumulators: the fp32
+        # output, else the (plain) bf16 one
+        yi = (y.float() if out_f32 is not None else y.float().bfloat16()).double().view(rows // stats_hw, stats_hw, Ncols)
         gn_stats[..., 0] += yi.sum(1)
         gn_stats[..., 1] += (yi * yi).sum(1)
     if out_bf16 is not None:

@@ -570,9 +570,11 @@ class Audit:
             prof_was = L.PROF.enabled
             if not prof_was:
                 L.PROF.start()
-            result = orig(*args, **kwargs)
+            try:
+                result = orig(*args, **kwargs)
+            finally:                        # a failed call must not leave the profiler on for the next one
+                fams = L.PROF.stop() if not prof_was else {}
             if not prof_was:
-                fams = L.PROF.stop()
                 family = next(iter(fams)) if len(fams) == 1 else entry
             torch.cuda.synchronize()
         else:
